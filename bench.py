@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Contract benchmark of the B200 path.
+"""Benchmark of the H100 (sm_90a) path.
 
     python bench.py --gpus N --steps K --warmup W                # images/sec, BASELINE.json configs[1] (N=1) / [2] (N>1)
     torchrun --nproc-per-node N ... bench.py --gpus N ...        # one rank per GPU over NCCL
@@ -13,7 +13,8 @@ One step = one pass of the hot path over one batch of synthetic input:
                    geocells are sharded across the ranks (second small all-gather of the per-candidate partials)   (configs[2])
   refiner        : B = 8192 queries (the same on every rank), P = 1M prototypes, D = 768, bank cell-sharded   (configs[4])
   train          : 128 four-view samples per rank, forward + backward + AdamW, NCCL gradient averaging        (configs[3])
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR also writes what the last timed step returned to its caller as
+DIR/<name>.npy (inputs are seeded, so two builds of the library can be compared output for output).
 """
 from __future__ import annotations
 
@@ -22,6 +23,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import time
 
 import numpy as np
@@ -44,24 +46,28 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d["bf16_tflops"], tflops_sustained=d["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # not measured: NVIDIA's data sheet for the H100 SXM at 700 W (HBM3 bandwidth, dense fp16 tensor rate); a power-limited
+    # card sustains less, so the "frac" figures below are lower bounds of the share of what the card can reach
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_sustained=989.0, source="NVIDIA H100 SXM data sheet (not measured)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
     def __init__(self, index: int):
-        self.index, self.proc, self.path = index, None, f"/tmp/pg_clocks_{os.getpid()}.csv"
+        self.index, self.proc, self.path = index, None, os.path.join(tempfile.gettempdir(), f"pg_clocks_{os.getpid()}.csv")
 
     def start(self):
-        try:
-            self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
-                                          "-lms", "200", "-i", str(self.index)], stdout=open(self.path, "w"),
-                                         stderr=subprocess.DEVNULL)
-        except OSError:
-            self.proc = None
+        with open(self.path, "w") as out:
+            try:
+                self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
+                                              "-lms", "200", "-i", str(self.index)], stdout=out, stderr=subprocess.DEVNULL)
+            except OSError:
+                self.proc = None
+        if self.proc is None:
+            os.remove(self.path)
 
     def stop(self):
         if self.proc is None:
@@ -71,9 +77,14 @@ class ClockSampler:
             self.proc.wait(timeout=5)
         except subprocess.TimeoutExpired:
             self.proc.kill()
+            self.proc.wait()
+        self.proc = None
+        with open(self.path) as f:
+            lines = f.readlines()
+        os.remove(self.path)
         sm, mx, reasons = [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
-        for line in open(self.path):
+        for line in lines:
             f = [x.strip() for x in line.split(",")]
             if len(f) < 9:
                 continue
@@ -88,6 +99,17 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["no samples"]}
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": max(mx), "reasons": sorted(reasons), "samples": len(sm)}
 
+    def sample(self, fn, enabled=True):
+        """fn() with the sampler running; the nvidia-smi process never outlives the call, whatever fn does."""
+        if not enabled:
+            return fn(), None
+        self.start()
+        try:
+            r = fn()
+        finally:
+            clocks = self.stop()
+        return r, clocks
+
 
 class Dist:
     """Process-group plumbing shared by the workloads (one rank per GPU, NCCL)."""
@@ -99,7 +121,7 @@ class Dist:
         self.rank = int(os.environ.get("RANK", "0"))
         self.local = int(os.environ.get("LOCAL_RANK", "0"))
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py: no CUDA device — the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+            raise SystemExit("bench.py: no CUDA device — the GPU path has no CPU fallback (use --impl reference for the CPU arm)")
         torch.cuda.set_device(self.local)
         self.dev = torch.device("cuda", self.local)
         if self.world > 1:
@@ -136,6 +158,14 @@ class Dist:
     def close(self):
         if self.world > 1:
             self.dist.destroy_process_group()
+
+
+def dump_outputs(directory, arrays):
+    """--dump-outputs: the arrays a caller of the timed path received in the last timed step, one float32 / float64 .npy each."""
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(directory, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
 
 
 def read_profile():
@@ -234,10 +264,13 @@ def run_infer(args):
         return ll.cpu(), cell.cpu(), out.loss.cpu()          # device -> host read of the step's result
 
     sampler = ClockSampler(D.local)
-    if rank == 0:
-        sampler.start()
-    ms, ms_by_rank, res = D.timed(step_device, args.steps, args.warmup)
-    clocks = sampler.stop() if rank == 0 else None
+    (ms, ms_by_rank, res), clocks = sampler.sample(lambda: D.timed(step_device, args.steps, args.warmup), rank == 0)
+    if args.dump_outputs and rank == 0:   # (256, 4, 1024) embeddings are 4 MB; everything else is smaller
+        ll_t, cell_t, out_t = res
+        dump_outputs(args.dump_outputs, dict(refined_lnglat=ll_t, refined_geocell=cell_t, embedding=out_t.embedding,
+                                             preds_lnglat=out_t.preds_LLH, preds_geocell=out_t.preds_geocell,
+                                             top_geocells=out_t.top5_geocells.indices, top_probs=out_t.top5_geocells.values,
+                                             loss=out_t.loss))
     e2e_steps = max(2, min(args.steps, 5))
     ms_e2e, e2e_by_rank, _ = D.timed(step_e2e, e2e_steps, 1)
 
@@ -289,20 +322,13 @@ def run_infer(args):
     gemm_ms, gemm_n = sum(v[0] for v in gemm.values()), sum(v[1] for v in gemm.values())
     attn_ms = fam.get("attention", (0.0, 0))[0]
     ach = GEMM_FLOP_PER_VIEW * views / (gemm_ms / 1e3) / 1e12
-    traffic, traffic_note = None, None
-    tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tp):
-        t = json.load(open(tp))
-        traffic, traffic_note = t.get("gemm_dram_bytes_per_launch"), t.get("how")
-    out["roofline"] = {"kernel": "gemm2_f16_kernel (tcgen05 GEMM, all projection/MLP launches of one step)", "bound": "tensor",
+    out["roofline"] = {"kernel": "gemm_f16_kernel (wgmma GEMM, all projection/MLP launches of one step)", "bound": "tensor",
                        "achieved": ach, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
-                       "frac": ach / peaks["tflops_sustained"], "traffic": traffic, "traffic_note": traffic_note,
-                       "peak_source": peaks["source"] + ", sustained bf16 cuBLAS figure (kernel timed inside a long step)",
+                       "frac": ach / peaks["tflops_sustained"], "traffic": None, "traffic_note": "not measured",
+                       "peak_source": peaks["source"],
                        "launches": gemm_n, "avg_launch_ms": gemm_ms / max(gemm_n, 1), "share_of_step": gemm_ms / total_ms}
     a_ach = ATTN_FLOP_PER_VIEW * views / (attn_ms / 1e3) / 1e12 if attn_ms else 0.0
-    attn_kernel = {None: "attention_fold_kernel", "fold": "attention_fold_kernel", "pair": "attention_pair_kernel",
-                   "split": "attention_split_kernel"}.get(os.environ.get("PG_ATTN_VARIANT"), "attention_kernel (first generation)")
-    out["roofline_attention"] = {"kernel": attn_kernel + " (tcgen05 QK^T / PV, softmax in between)", "bound": "tensor",
+    out["roofline_attention"] = {"kernel": "attention_kernel (wgmma QK^T / PV, softmax in between)", "bound": "tensor",
                                  "achieved": a_ach, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
                                  "frac": a_ach / peaks["tflops_sustained"], "share_of_step": attn_ms / total_ms}
     out["kernel_ms_per_step"] = {"gemm_ms": round(gemm_ms, 3), "attention_ms": round(attn_ms, 3),
@@ -368,7 +394,7 @@ def run_refiner(args):
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
 
     def step_device():
-        flush.zero_()                                       # the 0.4 GB shard at N = 8 would otherwise sit in the 126 MB L2 partly
+        flush.zero_()                                       # the 0.4 GB shard at N = 8 would otherwise sit in the 50 MB L2 partly
         return refiner(q, initial_preds=init, candidate_cells=candt, candidate_probs=probst)
 
     def step_e2e():
@@ -382,11 +408,10 @@ def run_refiner(args):
     def only_flush():
         flush.zero_()
     sampler = ClockSampler(D.local)
-    if rank == 0:
-        sampler.start()
-    ms_f, _, _ = D.timed(only_flush, args.steps, 2)
-    ms, ms_by_rank, res = D.timed(step_device, args.steps, args.warmup)
-    clocks = sampler.stop() if rank == 0 else None
+    (ms_f, (ms, ms_by_rank, res)), clocks = sampler.sample(
+        lambda: (D.timed(only_flush, args.steps, 2)[0], D.timed(step_device, args.steps, args.warmup)), rank == 0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(refined_lnglat=res[1], refined_geocell=res[2]))
     ms_e2e, e2e_by_rank, _ = D.timed(step_e2e, args.steps, 1)
     ms, ms_e2e = ms - ms_f, ms_e2e - ms_f
     lib = _lib.load()
@@ -474,10 +499,17 @@ def run_train(args):
         return out.loss
 
     sampler = ClockSampler(D.local)
-    if rank == 0:
-        sampler.start()
-    ms, ms_by_rank, loss = D.timed(lambda: step_with(px), args.steps, args.warmup)
-    clocks = sampler.stop() if rank == 0 else None
+    (ms, ms_by_rank, loss), clocks = sampler.sample(lambda: D.timed(lambda: step_with(px), args.steps, args.warmup), rank == 0)
+    if args.dump_outputs and rank == 0:
+        # what the step returns and what it updated: the loss, the head, and a fixed seeded sample of every parameter of the
+        # last encoder layer (trainable under both freeze policies), so a wrong tower backward shows in the dump
+        arrays = dict(loss=loss, cell_layer_weight=sg.cell_layer.weight, cell_layer_bias=sg.cell_layer.bias)
+        gs = torch.Generator().manual_seed(5)
+        for name, p in sg.base_model.vision_model.encoder.layers[-1].named_parameters():
+            flat = p.detach().reshape(-1)
+            idx = torch.randperm(flat.numel(), generator=gs)[:4096].sort().values
+            arrays["last_layer." + name] = flat[idx.to(flat.device)]
+        dump_outputs(args.dump_outputs, arrays)
     ms_e2e, _, _ = D.timed(lambda: step_with(px_host.to(dev, non_blocking=True)).cpu(), max(1, min(args.steps, 2)), 1)
     lib = _lib.load()
     lib.pg_profile_begin()
@@ -592,8 +624,7 @@ def cpu_baseline(sample_images: int):
 
 
 def run_reference(args):
-    """CPU arm: the oracle port of the reference path (the reference itself is Python under /root/reference and cannot travel to
-    the GPU box).  Same model, geocells, bank size and candidate counts as the GPU arm; one step = ONE four-view image, a
+    """CPU arm: the oracle port of the reference path (the reference itself is a separate Python project).  Same model, geocells, bank size and candidate counts as the GPU arm; one step = ONE four-view image, a
     bounded sample of the 256-image batch (the per-image cost of the fp32 CPU path does not depend on the batch size)."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -644,10 +675,14 @@ def main():
     ap.add_argument("--train-batch", type=int, default=128, help="train: four-view samples per GPU per step")
     ap.add_argument("--chunk-views", type=int, default=64)
     ap.add_argument("--all-trainable", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs applies to the GPU arm (--impl ours)")
         run_reference(args)
     elif args.workload == "refiner":
         run_refiner(args)

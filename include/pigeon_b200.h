@@ -1,5 +1,5 @@
 /*
- * pigeon_b200 — C ABI of the B200-native PIGEON inference hot path.
+ * pigeon_b200 — C ABI of the H100-native (sm_90a) PIGEON inference hot path.
  *
  * The reference (LukasHaas/PIGEON) has no FFI: its hot path sits behind Python nn.Module calls.  This header
  * is the seam a maintainer binds underneath those modules (ctypes stub in INTEGRATION.md); every entry point
@@ -104,7 +104,7 @@ int pg_head_forward(const float* emb, int32_t B, int32_t V, int32_t D, const voi
                     float* pooled, float* logits, float* probs, int64_t* pred_cell, double* pred_lnglat,
                     float* topk_val, int64_t* topk_idx, void* stream);
 /* Measurement / deployment switch of pg_head_forward for this process: 0 (default) = three kernels (view mean + split,
- * tcgen05 GEMM + bias, softmax / arg-max / top-k); 1 = ONE kernel doing all of it (D % 64 == 0 and C <= 6144, otherwise the
+ * wgmma GEMM + bias, softmax / arg-max / top-k); 1 = ONE kernel doing all of it (D % 64 == 0 and C <= 6144, otherwise the
  * three-kernel sequence runs): the view mean and the hi/lo split happen in the GEMM's A-operand producer warps and the CTA
  * that completes a block of 128 samples last normalises its rows.  Same results to fp32 summation order. */
 int pg_head_set_fused(int32_t on);
@@ -312,7 +312,7 @@ enum {
   PG_EPI_F32_BIAS_RESID = 2, /* out f32 += A W^T + bias                        (out_proj, mlp.fc2) */
   PG_EPI_F32_BIAS = 3        /* out f32 = A W^T + bias (bias may be NULL)                          */
 };
-/* D[M,N] = A[M,K] (fp16, row stride lda) * W[N,K]^T (fp16, row stride ldw), fp32 accumulate on tcgen05. */
+/* D[M,N] = A[M,K] (fp16, row stride lda) * W[N,K]^T (fp16, row stride ldw), fp32 accumulate on wgmma. */
 int pg_gemm_f16(const void* a, int32_t lda, const void* w, int32_t ldw, void* out, int32_t ldo, const float* bias,
                 int32_t M, int32_t N, int32_t K, int32_t epilogue, void* stream);
 /* pg_gemm_f16 with bf16 operands (operand_bf16 != 0: BOTH a and w are bf16 — the tensor cores reject mixed pairs) and,
@@ -321,8 +321,8 @@ int pg_gemm_f16(const void* a, int32_t lda, const void* w, int32_t ldw, void* ou
 int pg_gemm_ex(const void* a, int32_t lda, const void* w, int32_t ldw, void* out, int32_t ldo, const float* bias,
                const float* resid, int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t operand_bf16, void* stream);
 /* D[M, N] (+)= a^T w with BOTH operands stored contraction-major: a [K, lda] (M contiguous), w [K, ldw] (N contiguous) —
- * the weight-gradient form dW = dY^T X fed from row-major activations (MN-major UMMA operands, no transposes).
- * M % 64 == 0, M > 128, N % 256 == 0; epilogue PG_EPI_F32_BIAS (overwrite) or PG_EPI_F32_BIAS_RESID (accumulate in place). */
+ * the weight-gradient form dW = dY^T X fed from row-major activations (MN-major wgmma operands, no transposes).
+ * M > 128, N % 256 == 0, lda and ldw multiples of 8 (other shapes are rejected); epilogue PG_EPI_F32_BIAS (overwrite) or PG_EPI_F32_BIAS_RESID (accumulate in place). */
 int pg_gemm_tn(const void* a, int32_t lda, const void* w, int32_t ldw, float* out, int32_t ldo, int32_t M, int32_t N,
                int32_t K, int32_t accumulate, int32_t operand_bf16, void* stream);
 /* LayerNorm over the last dim: x f32 [rows, hidden] -> y fp16 [rows, hidden]. */
@@ -330,10 +330,8 @@ int pg_layernorm_f16(const float* x, void* y, const float* gamma, const float* b
                      float eps, void* stream);
 /* softmax(q k^T / 8) v per (view, head); qkv fp16 [n_views*seq, 3*heads*64] -> out fp16 [n_views*seq, heads*64]. */
 int pg_attention_f16(const void* qkv, void* out, int32_t n_views, int32_t seq, int32_t heads, void* stream);
-/* Measurement aid: the same op with the kernel chosen explicitly.  variant 0 = "pair" kernel (persistent, two query tiles per
- * CTA, KV blocks of 128, Q in tensor memory; poly = eighths of the exponentials evaluated on the FMA pipe, < 0 = default),
- * variant 1 = first-generation kernel (one tile per CTA, KV blocks of 32), variant 2 = "split" kernel (the pair kernel with
- * sixteen softmax warps: two independent column halves per S block, merged in the epilogue).  lse2 may be NULL. */
+/* The same op with the optional lse2 side output (may be NULL).  `variant` (0..3) and `poly` selected among several forward
+ * kernels in earlier versions of this ABI; the sm_90a library has one wgmma kernel, and every variant runs it. */
 int pg_attention_f16_variant(const void* qkv, void* out, float* lse2, int32_t n_views, int32_t seq, int32_t heads,
                              int32_t variant, int32_t poly, void* stream);
 /* Same, also writing lse2 f32 [n_views*heads, seq] (log2-sum-exp of the scaled logits) for the backward pass. */

@@ -1,4 +1,4 @@
-"""pigeon_b200 — B200-native (sm_100a) implementation of PIGEON's image-geolocation inference hot path.
+"""pigeon_b200 — H100-native (sm_90a) implementation of PIGEON's image-geolocation inference hot path.
 
     CLIPEmbedding  (reference models/clip_embedder.py)   ViT-L/14-336 forward + token mean
     SuperGuessr    (reference models/super_guessr.py)    geocell head: Linear + softmax + argmax + top-k (+ CE loss)

@@ -1,7 +1,6 @@
-"""In-tree nvcc build of libpigeon_b200.so (sm_100a only).
+"""In-tree nvcc build of libpigeon_b200.so (sm_90a only).
 
-The shared object is built next to the sources so that it travels with a snapshot of the repo
-(the GPU boxes have no persistent JIT cache).  `build()` is idempotent: it rebuilds only when a
+The shared object is built next to the sources so that it travels with a snapshot of the repo.  `build()` is idempotent: it rebuilds only when a
 source, header or flag changed (content hash), and never needs a GPU (nvcc cross-compiles).
 """
 from __future__ import annotations
@@ -22,27 +21,23 @@ OBJ_DIR = CSRC / "build"
 
 SOURCES = [
     "tma_host.cu",
-    "gemm_tcgen05.cu",
-    "gemm2_tcgen05.cu",
-    "attention_tcgen05.cu",
-    "attention_pair_tcgen05.cu",
-    "attention_split_tcgen05.cu",
-    "attention_fold_tcgen05.cu",
+    "gemm_wgmma.cu",
+    "attention_wgmma.cu",
     "nccl_gather.cu",
     "vit_misc.cu",
     "head.cu",
-    "head_fused_tcgen05.cu",
+    "head_fused_wgmma.cu",
     "refiner.cu",
     "train.cu",
     "preprocess.cu",
     "train_vit.cu",
-    "attention_bwd_tcgen05.cu",
+    "attention_bwd_wgmma.cu",
     "vit_train_capi.cu",
     "capi.cu",
 ]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -52,7 +47,7 @@ NVCC_FLAGS = [
 def _nvcc() -> str:
     exe = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(exe):
-        raise RuntimeError("nvcc not found: pigeon_b200 needs the CUDA 12.9 toolkit to build its sm_100a kernels")
+        raise RuntimeError("nvcc not found: pigeon_b200 needs the CUDA 12.9 toolkit to build its sm_90a kernels")
     return exe
 
 
@@ -78,7 +73,7 @@ def is_current() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every CUDA source for sm_100a and link libpigeon_b200.so in-tree."""
+    """Compile every CUDA source for sm_90a and link libpigeon_b200.so in-tree."""
     stamp = OBJ_DIR / "digest.txt"
     digest = _digest()
     if not force and LIB_PATH.exists() and stamp.exists() and stamp.read_text() == digest:
@@ -99,7 +94,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
     tmp = LIB_PATH.with_suffix(".so.tmp")
-    cmd = [nvcc, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-shared", "-o", str(tmp), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a",
            "-cudart", "static", "-Xlinker", "--exclude-libs,ALL", "-ldl"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

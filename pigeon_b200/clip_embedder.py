@@ -1,4 +1,4 @@
-"""CLIPEmbedding — the reference's CLIP ViT-L/14-336 image embedder (models/clip_embedder.py) with the B200 tower behind it.
+"""CLIPEmbedding — the reference's CLIP ViT-L/14-336 image embedder (models/clip_embedder.py) with the H100 tower behind it.
 
 Same constructor arguments (`model_name, device='cuda', load_checkpoint=False, panorama=False`), same call
 (`embedder(image) -> Tensor[N, hidden]`), same result: the mean over ALL tokens of `last_hidden_state`

@@ -1,4 +1,4 @@
-// Internal (C++) interface of the tcgen05 attention core; the C ABI in capi.cu wraps it.
+// Internal (C++) interface of the wgmma attention core; the C ABI in capi.cu wraps it.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -9,27 +9,7 @@ namespace pg {
 int attention_f16(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream,
                   float* lse2 = nullptr);
 
-// Second-generation forward kernel (attention_pair_tcgen05.cu): persistent, two query tiles per CTA, KV blocks of 128.
-// poly = eighths of the exponentials evaluated on the FMA pipe (0..3).  attention_f16 dispatches to it by default.
-int attention_pair_f16(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream, float* lse2,
-                       int poly);
-
-// Third-generation forward kernel (attention_split_tcgen05.cu): the pair kernel's job structure with SIXTEEN softmax warps
-// (every S block split into two independent column halves with their own accumulators, merged in the epilogue; Q in smem).
-int attention_split_f16(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream, float* lse2,
-                        int poly);
-
-// Fourth-generation forward kernel (attention_fold_tcgen05.cu): the pair kernel with the softmax scale, reference subtraction
-// and row sum moved into the MMAs (extra k-step / ones-column accumulator); rows whose fp16 P overflows are repaired exactly.
-int attention_fold_f16(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream, float* lse2,
-                       int poly);
-
-// Explicit kernel choice for A/B measurements: variant 0 = pair kernel, 2 = split kernel, 3 = fold kernel (poly in eighths, < 0 = default), 1 = first-generation
-// kernel (poly 0 / 4 / 2 = none / every 4th / every 2nd group).
-int attention_f16_variant(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream, float* lse2,
-                          int variant, int poly);
-
-// Backward of the attention core (attention_bwd_tcgen05.cu).
+// Backward of the attention core (attention_bwd_wgmma.cu).
 //   qkv f16 / qkv_bf16 [n_views*seq, 3*heads*64] (same values, two operand types), d_out_bf16 [n_views*seq, heads*64],
 //   lse2 / delta f32 [n_views*heads, seq]  ->  dqkv bf16 [n_views*seq, 3*heads*64]
 int attention_backward(const void* qkv_f16, const void* qkv_bf16, const void* d_out_bf16, const float* lse2,

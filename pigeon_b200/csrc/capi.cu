@@ -236,7 +236,7 @@ int pg_head_forward(const float* emb, int32_t B, int32_t V, int32_t D, const voi
   const int sms = sm_count();
   if (sms < 0) return 1;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  // pg_head_set_fused(1): one kernel (view mean + split -> tcgen05 GEMM -> bias -> softmax / arg-max / top-k) whenever the
+  // pg_head_set_fused(1): one kernel (view mean + split -> wgmma GEMM -> bias -> softmax / arg-max / top-k) whenever the
   // shape allows; the default is the three-kernel sequence, which is faster at the batch sizes of this path (DESIGN.md 5.4)
   if (head_fused_on() && head_fused_supported(B, V, D, C, k) && (reinterpret_cast<uintptr_t>(emb) & 15) == 0)
     return head_fused_forward(emb, B, V, D, w3, bias, centroids, C, k, workspace, pooled, logits, probs,
@@ -512,7 +512,8 @@ int pg_attention_f16_variant(const void* qkv, void* out, float* lse2, int32_t n_
                              int32_t variant, int32_t poly, void* stream) {
   if (!qkv || !out) { set_last_error("pg_attention_f16_variant: null argument"); return 1; }
   if (variant < 0 || variant > 3) { set_last_error("pg_attention_f16_variant: variant %d not in {0, 1, 2, 3}", variant); return 1; }
-  return attention_f16_variant(qkv, out, n_views, seq, heads, reinterpret_cast<cudaStream_t>(stream), lse2, variant, poly);
+  (void)poly;   // one kernel on sm_90a: every variant number of the ABI runs it
+  return attention_f16(qkv, out, n_views, seq, heads, reinterpret_cast<cudaStream_t>(stream), lse2);
 }
 
 }  // extern "C"

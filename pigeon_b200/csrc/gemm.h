@@ -1,4 +1,4 @@
-// Internal (C++) interface of the tcgen05 GEMM; the C ABI in capi.cu wraps it.
+// Internal (C++) interface of the wgmma GEMM; the C ABI in capi.cu wraps it.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -35,8 +35,8 @@ struct GemmProblem {
   const float* resid;   // EPI_F32_BIAS_RESID: residual read from here instead of `out` (same ldo); nullptr = in place
   void* aux;            // fp16 [M, ldo]: pre-activation read by EPI_BF16_DGELU / written by EPI_F16_BIAS_QGELU_SAVE
   // Both operands stored with the CONTRACTION index outermost: a = [K, lda] (M contiguous), w = [K, ldw] (N contiguous),
-  // i.e. D = a^T w — the weight-gradient form (dW = dY^T X) fed straight from row-major activations as MN-major UMMA
-  // operands.  2-CTA kernel only (M > 128, N % 256 == 0, M % 64 == 0).
+  // i.e. D = a^T w — the weight-gradient form (dW = dY^T X) fed straight from row-major activations as MN-major wgmma
+  // operands (M > 128, N % 256 == 0).
   int mn_major;
   // LayerNorm-folded epilogues: stats float2 [M, K / 128] (consumer, read) or [M, N / 128] (producer, written);
   // colsum fp32 [N] = row sums of the (gamma-scaled, fp16-rounded) weight; ln_eps of the LayerNorm.

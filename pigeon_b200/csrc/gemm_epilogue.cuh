@@ -1,5 +1,6 @@
-// Shared epilogue of the tcgen05 GEMM kernels (1-CTA and 2-CTA): TMEM accumulator tile (128 rows x BLOCK_N fp32
-// columns per CTA) -> bias / activation / residual -> global.  Included by gemm_tcgen05.cu and gemm2_tcgen05.cu.
+// Shared epilogue of the wgmma kernels (gemm_wgmma.cu, head_fused_wgmma.cu): the warpgroup parks its fp32 accumulator
+// fragments in a shared-memory tile (128 rows x 128 columns, rows padded by 4 floats), then each warp takes 32 rows of it
+// -> bias / activation / residual -> global.
 #pragma once
 #include "gemm.h"
 #include "ptx.cuh"
@@ -9,6 +10,9 @@
 namespace pg {
 
 constexpr int kStageWarpBytes = 32 * 128;   // per epilogue warp: 32 rows x 128 B, 16-byte pieces XOR-swizzled by (row & 7)
+constexpr int kEpiTileN = 128;                       // columns of the accumulator tile
+constexpr int kAccLdBytes = (kEpiTileN + 4) * 4;     // padded row: a warp reading one row per lane (16 bytes each) hits no bank twice
+constexpr int kAccTileBytes = 128 * kAccLdBytes;
 
 struct GemmArgs {
   int M, N, K;
@@ -18,11 +22,10 @@ struct GemmArgs {
   // EPI_F32_ROWMAP: output row = rowmap_mul * (row / rowmap_div) + row % rowmap_div + rowmap_add
   int rowmap_div, rowmap_mul, rowmap_add;
   int vec_ok;  // output rows are 16-byte aligned -> vector stores allowed
-  uint32_t idesc_fmt;  // A/B format bits of the instruction descriptor (0 = fp16, bf16 otherwise)
+  int operand_bf16;    // A and W hold bf16 instead of fp16
   const float* resid;  // residual source of EPI_F32_BIAS_RESID (== out when updating in place)
   void* aux;           // EPI_BF16_DGELU: fc1 pre-activation (fp16, read);  EPI_F16_BIAS_QGELU_SAVE: where to keep it (written)
-  int mn_major;        // operands are [K, M] / [K, N] (MN-major UMMA operands), see GemmProblem::mn_major
-  uint32_t mn_lbo, mn_sbo;   // descriptor strides of the MN-major operand tiles (bytes)
+  int mn_major;        // operands are [K, M] / [K, N] (MN-major wgmma operands), see GemmProblem::mn_major
   float* stats;         // LayerNorm-folded epilogues: float2 [M, stats_slots] partial (sum, sum of squares) per 128 columns
   int stats_slots;      // producer: N / 128; consumer: K / 128
   const float* colsum;  // consumer: fp32 [N] row sums of the folded weight
@@ -49,10 +52,22 @@ __device__ __forceinline__ uint32_t pack_bf16x2_rn(float lo, float hi) {
   return r;
 }
 
+// Accumulator fragment of one m64 wgmma block (wgmma.cuh layout) -> the shared accumulator tile; `blk_row0` = tile row of the
+// block's first row, `acc_s` = shared address of the tile.
+__device__ __forceinline__ void store_acc_fragment(uint32_t acc_s, int blk_row0, const float (&d)[kEpiTileN / 2], int warp_in_group,
+                                                   int lane) {
+  const uint32_t r0 = acc_s + (uint32_t)(blk_row0 + 16 * warp_in_group + (lane >> 2)) * kAccLdBytes + (uint32_t)(lane & 3) * 8;
+#pragma unroll
+  for (int j = 0; j < kEpiTileN / 8; ++j) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + j * 32), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + 8 * kAccLdBytes + j * 32), "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
+  }
+}
+
 // One epilogue warp's share of one output tile: rows [warp_row0, warp_row0 + 32), tile columns [c_begin, c_end).
-//   t_row  : TMEM address of this warp's lane quarter at the accumulator stage's first column
-//   stage  : this warp's private staging buffer (kStageWarpBytes)
-// Per chunk of CHUNK columns (128 bytes of output per row): TMEM -> registers (thread = row) -> bias / activation ->
+//   acc_row_s : shared address of this warp's first row (column 0) in the accumulator tile
+//   stage     : this warp's private staging buffer (kStageWarpBytes)
+// Per chunk of CHUNK columns (128 bytes of output per row): accumulator tile -> registers (thread = row) -> bias / activation ->
 // smem staging (32 rows x 128 B, pieces swizzled: conflict-free both ways) -> coalesced global phase in which 8 lanes
 // cover one 128-byte row segment (4 rows per instruction).  For the residual epilogue the 16-byte pieces a lane will
 // update are fetched ONE CHUNK AHEAD so that their HBM latency hides behind the current chunk's work.
@@ -67,9 +82,9 @@ struct EpiTraits {
   static constexpr int kElt = kF16Out ? 2 : 4;   // EPI_BF16_DGELU stages fp32 (CHUNK 32) and stores 2-byte elements
 };
 
-// L2 eviction policies (createpolicy): the fp32 residual stream (read-modify-write, 4.8 GB per launch at the bench shape) and
-// the fp16 copy are touched once per kernel and are far larger than the 126 MB L2 — marked evict_first so that they do not
-// push out the A operand, which the four CTA pairs of a 256-row block share through L2.
+// L2 eviction policies (createpolicy): the fp32 residual stream (read-modify-write) and
+// the fp16 copy are touched once per kernel and are far larger than the 50 MB L2 — marked evict_first so that they do not
+// push out the A operand, which the CTAs of one 128-row block share through L2.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -108,7 +123,7 @@ __device__ __forceinline__ void load_residual(const GemmArgs& args, float4 (&res
 }
 
 template <int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmArgs& args, uint32_t t_row, uint8_t* stage, int warp_row0,
+__device__ __forceinline__ void epilogue_tile(const GemmArgs& args, uint32_t acc_row_s, uint8_t* stage, int warp_row0,
                                               int tile_col0, int c_begin, int c_end, int lane) {
   constexpr bool kF16Out = EpiTraits<EPI>::kF16Out;
   constexpr int CHUNK = EpiTraits<EPI>::CHUNK;
@@ -161,14 +176,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmArgs& args, uint32_t t_r
       const int ncol0 = col0 + CHUNK;
       if (c0 + CHUNK < c_end && args.vec_ok && ncol0 + CHUNK <= args.N) load_residual<EPI>(args, res_next, warp_row0, ncol0, lane, pol_stream);
     }
-    uint32_t r[CHUNK];
     __syncwarp();
-#pragma unroll
-    for (int h = 0; h < CHUNK / 32; ++h) tmem_ld32(t_row + c0 + 32 * h, *reinterpret_cast<uint32_t(*)[32]>(&r[32 * h]));
-    tmem_ld_wait();
     float v[CHUNK];
 #pragma unroll
-    for (int i = 0; i < CHUNK; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < CHUNK / 4; ++i) {
+      const float4 t = lds_f4(acc_row_s + (uint32_t)lane * kAccLdBytes + (uint32_t)(c0 + 4 * i) * 4);
+      v[4 * i + 0] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+    }
     if (kLn) {   // LayerNorm folded: rstd * acc + (-rstd * mu) * colsum + bias, two FMAs per element
       // (N is a multiple of the chunk and bias != nullptr: checked at launch)
       const float4* c4 = reinterpret_cast<const float4*>(args.colsum + col0);

@@ -1,4 +1,4 @@
-// Geocell head around the tcgen05 GEMM: restates reference models/super_guessr.py:437 (4-view mean),
+// Geocell head around the wgmma GEMM: restates reference models/super_guessr.py:437 (4-view mean),
 // :447-448 (cell_layer Linear + softmax), :454-455 (argmax + centroid lookup), :459 (top-k).
 //
 // The Linear is evaluated on the fp16 tensor-core path at fp32-faithful accuracy by an error-compensated

@@ -9,7 +9,7 @@ int weight_split(const float* w, void* w3_f16, int C, int D, cudaStream_t stream
 int softmax_topk(const float* logits, float* probs, long long* pred_cell, double* pred_lnglat, float* topk_val,
                  long long* topk_idx, const double* centroids, int B, int C, int k, cudaStream_t stream);
 
-// The three steps above as one kernel (head_fused_tcgen05.cu): view mean + split in the A-operand producers, tcgen05 GEMM,
+// The three steps above as one kernel (head_fused_wgmma.cu): view mean + split into the A operand tiles, wgmma GEMM,
 // bias, and softmax / arg-max / top-k by the CTA that completes a block of 128 samples last.  `tickets`: int per block.
 bool head_fused_supported(int B, int V, int D, int C, int k);
 size_t head_fused_workspace_bytes(int B);

@@ -1,4 +1,4 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 // Everything here is a 1:1 wrapper over one PTX instruction; the kernels in this directory are
 // written against these wrappers only (no CUTLASS / CuTe templates).
 #pragma once
@@ -8,10 +8,12 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "wgmma.cuh"
+
 namespace pg {
 
 #ifndef PG_SPIN_LIMIT
-// A dead-locked mbarrier wait traps instead of hanging the GPU (the box is shared; a hang is a strike).
+// A dead-locked mbarrier wait traps instead of hanging the GPU.
 #define PG_SPIN_LIMIT (1u << 26)
 #endif
 
@@ -66,9 +68,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 
 // A dead-locked wait traps (see PG_SPIN_LIMIT).  The report (block, thread, barrier address, parity) is compiled in only
 // with -DPG_DEADLOCK_REPORT (PG_NVCC_EXTRA="-DPG_DEADLOCK_REPORT" python -m pigeon_b200._build --force): inlined at every
-// wait it costs ~50 instructions per site and instruction-cache misses in the attention kernels (dozens of waits), and as
-// a __noinline__ function it made ptxas hold EVERY warp role to the smallest setmaxnreg budget of the kernel (measured:
-// the softmax warps of attention_pair_kernel spilled their loop state at 77 registers instead of using 132).
+// wait it costs ~50 instructions per site.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -97,6 +97,17 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       " [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0),
       "r"(c1)
+      : "memory");
+}
+
+// 3-D tiled load: c0 = innermost coordinate, c2 = outermost.
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
+                                            int32_t c0, int32_t c1, int32_t c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0),
+      "r"(c1), "r"(c2)
       : "memory");
 }
 
@@ -140,147 +151,41 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* gsrc, uint32_t byte
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, commit, MMA, TMEM load/store
+// wgmma: fences, group commit / wait, shared-memory matrix descriptor (the MMA wrappers are in wgmma.cuh)
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// Arrives (count 1) on the mbarrier once all previously issued tcgen05.mma of this thread retired.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
+// Orders register / shared-memory accesses of the warpgroup before the next wgmma.mma_async.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// Waits until at most N committed groups of this warpgroup are still in flight.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// Shared-memory matrix descriptor (SM100 "version 1"), see DESIGN.md §kernels for the field map.
+// Shared-memory matrix descriptor of a 128-byte-swizzled operand tile (1024-byte aligned):
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1
-//   bits [61,64) layout: 0 none, 2 = 128-byte swizzle, 4 = 64-byte, 6 = 32-byte
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes, uint32_t layout) {
+//   bits [32,46) stride byte offset >> 4   bits [62,64) swizzle: 1 = 128 bytes
+// K-major tile (rows of 64 halves): stride offset = distance between 8-row groups (1024); a K step of 16 halves = +32 bytes.
+// MN-major tile (64 contiguous M/N halves per contraction row): stride offset = distance between groups of 8 contraction
+// rows (1024), leading offset = distance between 64-column blocks of M/N.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout & 7u) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-constexpr uint32_t kLayoutSw128 = 2;
 
-// Instruction descriptor for kind::f16 with fp16 A/B and fp32 accumulate.
-//   [4,6) D format (1 = f32)  [7,10) A format (0 = f16)  [10,13) B format (0 = f16)
-//   [15] A major (0 = K)      [16] B major (0 = K, 1 = MN)
-//   [17,23) N >> 3            [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn,
-                                                      uint32_t b_mn) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (a_mn << 15) | (b_mn << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+// Named barrier over `threads` threads of the block (barrier 0 is __syncthreads).
+template <int ID>
+__device__ __forceinline__ void named_barrier(int threads) {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "r"(threads) : "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// TMEM -> registers: the warp reads its own 32-lane quarter, 32 consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// registers -> TMEM, 16 consecutive 32-bit columns of the warp's own lane quarter.
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// Packed fp32 pair arithmetic (Blackwell FFMA2 / FADD2: two lanes of fp32 per instruction).
+// fp32 pair FMA: two independent fused multiply-adds (sm_90 has no packed-fp32 instruction).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)),
-        "l"(*reinterpret_cast<unsigned long long*>(&c)));
-  return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  unsigned long long d;
-  asm("add.rn.f32x2 %0, %1, %2;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 fsub2(float2 a, float2 b) {
-  unsigned long long d;
-  asm("sub.rn.f32x2 %0, %1, %2;"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&d);
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {

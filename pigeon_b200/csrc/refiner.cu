@@ -119,7 +119,7 @@ scan_kernel(const RefinerBank bank, const float* __restrict__ q, const long long
 // Cell-major scan (v2).  (query, candidate) pairs are counting-sorted by geocell; one CTA per geocell then reads
 // that cell's prototype segment from HBM ONCE (re-reads per 8-query chunk come from L2) and scores every pair of the
 // cell against it.  Per warp a 4-prototype x 8-query register tile: prototype rows stay in registers, the 8 query
-// rows sit in shared memory interleaved in pairs so that one FFMA2 (packed fp32) advances two queries' dot products.
+// rows sit in shared memory interleaved in pairs so that one float2 FMA (ffma2) advances two queries' dot products.
 // Algorithmic bytes: sum over touched cells of P_c * D * 4, each once.
 // ------------------------------------------------------------------------------------------------
 constexpr int kQT = 8;  // queries per chunk
@@ -229,7 +229,7 @@ cell_major_scan_kernel(const RefinerBank bank, const float* __restrict__ q, cons
     const int nq = min(QS, n_pairs - c0);
     const int nch = (nq + kQT - 1) / kQT;
     __syncthreads();
-    // stage the queries, two interleaved per float4 (see the FFMA2 loop):
+    // stage the queries, two interleaved per float4 (see the ffma2 loop):
     //   qs[(((ch * NV4 + i) * (kQT/2) + qp) * 2 + h) * 32 + lane] = for h = 0: (qA[4c], qB[4c], qA[4c+1], qB[4c+1]),
     //   for h = 1 the same for elements 4c+2, 4c+3;  A = ch*8 + 2qp, B = A + 1, c = lane + 32 i
     for (int idx = threadIdx.x; idx < nch * NV4 * (kQT / 2) * 32; idx += blockDim.x) {
@@ -290,7 +290,7 @@ cell_major_scan_kernel(const RefinerBank bank, const float* __restrict__ q, cons
       const bool p_ok = (p0 + (lane >> 3)) < hi;
 
       for (int ch = 0; ch < nch; ++ch) {
-        // d^2 = |p|^2 + |q|^2 - 2 p.q (the form torch.cdist itself uses beyond 25 rows): one FFMA2 per two (p, q)
+        // d^2 = |p|^2 + |q|^2 - 2 p.q (the form torch.cdist itself uses beyond 25 rows): one ffma2 per two (p, q)
         // element pairs.
         float2 acc[kPT][kQT / 2];
 #pragma unroll
@@ -385,22 +385,21 @@ cell_major_scan_kernel(const RefinerBank bank, const float* __restrict__ q, cons
 }
 
 // ------------------------------------------------------------------------------------------------
-// Tile scan (v4).  The cell-major kernel above is latency-bound on its prototype stream: a warp requests 12 KB, waits for
-// it, computes, and only then requests again (ncu: issue slots 36 %, DRAM 25 %).  Here the stream is decoupled from the
-// arithmetic:
+// Tile scan (v4).  In the cell-major kernel above a warp requests 12 KB of its prototype stream, waits for it, computes, and
+// only then requests again.  Here the stream is decoupled from the arithmetic:
 //   * persistent CTAs (one per SM, 8 consumer warps + 1 producer warp); the work is the list of 16-prototype TILES of all
 //     touched (geocell, query pass) pairs in cell order, cut into gridDim.x equal contiguous ranges (no tail, no wave
 //     quantisation); a geocell that straddles two ranges is merged through a 64-bit atomicMin on (d2 bits, prototype);
 //   * the producer warp copies each tile (16 rows x D floats) into a shared-memory ring with one cp.async.bulk per row,
 //     completion on an mbarrier, and pulls the tiles kPrefetchTiles further ahead into L2 (cp.async.bulk.prefetch.L2),
 //     so HBM latency is hidden by L2 depth rather than by shared memory;
-//   * up to QS queries of the geocell sit in shared memory for the whole pass, interleaved in pairs (one FFMA2 advances
+//   * up to QS queries of the geocell sit in shared memory for the whole pass, interleaved in pairs (one ffma2 advances
 //     two queries); the 8 consumer warps split D eight ways, each computing a 16 x QS block of partial dot products with
 //     a 2-prototype x NCH-pair register tile per thread (lanes = 8 prototype groups x 4 query groups: every LDS.128 is a
 //     single conflict-free wavefront thanks to the 16-byte row padding), then add the eight partials in a fixed order
 //     through shared memory -> d2 = |p|^2 + |q|^2 - 2 p.q with |p|^2 precomputed per bank (proto_sqnorm).
 // Every (prototype, query) distance is computed by the same instruction sequence wherever the tile lands, so a sharded bank
-// reproduces the single-GPU selections bit for bit.  FP32-FMA floor at cfg5: 0.5 ms; HBM floor 0.47 ms.
+// reproduces the single-GPU selections bit for bit.
 // ------------------------------------------------------------------------------------------------
 constexpr int kTP = 16;                 // prototypes per tile = one ring stage
 constexpr int kTileWarps = 8;           // consumer warps (D split 8 ways)
@@ -695,18 +694,16 @@ tile_scan_kernel(const RefinerBank bank, const float* __restrict__ q, const int*
 }
 
 // ------------------------------------------------------------------------------------------------
-// Slab scan (v5).  Measured on this GPU (tools/ubench/fp32_lds.cu): shared memory delivers 128 bytes per clock per SM to the
-// registers whatever the broadcast pattern — an LDS.128 costs four LSU cycles — and FFMA2 retires 128 FMA per clock per SM.
-// A kernel whose operands come from shared memory is therefore FMA-bound only from 4 FMA per delivered float upwards; the
-// tile scan's 2 x 2NCH register tile delivers 1.5 (ncu: LSU wavefronts 76 %, FMA pipe 33 %), the cell-major kernel 4 but
-// pays a 31-shuffle reduction per 32 results.  This kernel uses the 8-prototype x 8-query outer-product tile (4 FMA per
-// float: 79 % of the FMA peak in the micro-benchmark) without any cross-lane reduction:
+// Slab scan (v5).  A kernel whose operands come from shared memory does more arithmetic per delivered float the larger its
+// register tile: the tile scan's 2 x 2NCH tile does 1.5 FMA per float, the cell-major kernel 4 but it pays a 31-shuffle
+// reduction per 32 results.  This kernel uses the 8-prototype x 8-query outer-product tile (4 FMA per float) without any
+// cross-lane reduction:
 //   * a warp owns a SLAB of 64 prototypes (lanes = 8 prototype groups x 4 query groups; thread = 8 prototypes x up to 4
 //     query pairs, accumulators in registers over the whole embedding), a CTA up to 8 consecutive slabs of one geocell;
 //   * the embedding dimension is streamed in chunks of 32 floats: one TMA box of [256 prototypes x 128 bytes] per half tile
 //     (tensor map over the bank, 128-byte swizzle -> conflict-free LDS.128 of 8 rows), 3 stages of 64 KB, mbarrier ring;
 //   * the query chunk [32 queries x 32 floats] is gathered by the consumer threads one chunk ahead (registers -> double
-//     buffer, pairs interleaved for FFMA2, rows padded by 16 bytes);
+//     buffer, pairs interleaved for ffma2, rows padded by 16 bytes);
 //   * d2 = |p|^2 + |q|^2 - 2 p.q, minimum over the thread's prototypes, three shuffles across the prototype groups, one
 //     packed atomicMin per (warp, query): partition-independent like the tile scan.
 // Work list = slabs of all touched (geocell, query pass) pairs, cut into gridDim.x equal contiguous ranges.

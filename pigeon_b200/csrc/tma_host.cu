@@ -66,6 +66,31 @@ int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t
   return 0;
 }
 
+// 16-bit [views, rows_per_view, cols] (ld_elems elements per row, views contiguous): box [1, box_rows, box_cols].  A box that
+// runs past a view's last row is zero-filled instead of reading the next view's rows.
+int make_tmap_f16_3d(CUtensorMap* out, const void* base, uint64_t views, uint64_t rows_per_view, uint64_t cols, uint64_t ld_elems,
+                     uint32_t box_rows, uint32_t box_cols) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) {
+    set_last_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
+    return 1;
+  }
+  cuuint64_t gdim[3] = {cols, rows_per_view, views};
+  cuuint64_t gstride[2] = {ld_elems * 2, rows_per_view * ld_elems * 2};
+  cuuint32_t box[3] = {box_cols, box_rows, 1};
+  cuuint32_t estride[3] = {1, 1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), gdim, gstride, box, estride,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled (3-D) failed: CUresult %d (views=%llu rows=%llu cols=%llu ld=%llu box=%ux%u)", (int)r,
+                   (unsigned long long)views, (unsigned long long)rows_per_view, (unsigned long long)cols,
+                   (unsigned long long)ld_elems, box_rows, box_cols);
+    return 1;
+  }
+  return 0;
+}
+
 // fp32 [rows, cols] row-major (ld_elems floats per row), box [box_rows, box_cols] with box_cols * 4 == 128 bytes, 128-byte swizzle.
 int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                      uint32_t box_rows, uint32_t box_cols) {

@@ -13,6 +13,10 @@ namespace pg {
 int make_tmap_f16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                      uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols);
 
+// 16-bit [views, rows_per_view, cols] with a [1, box_rows, box_cols] tile: rows past a view's end are zero-filled.
+int make_tmap_f16_3d(CUtensorMap* out, const void* base, uint64_t views, uint64_t rows_per_view, uint64_t cols,
+                     uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols);
+
 int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                      uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols);
 

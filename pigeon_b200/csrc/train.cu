@@ -129,7 +129,7 @@ int adamw_step(float* p, const float* g, float* m, float* v, long n, double lr, 
                double weight_decay, long step, double grad_scale, cudaStream_t stream) {
   const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
   long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   ProfScope prof("train_adamw", stream);
   adamw_kernel<<<(int)blocks, 256, 0, stream>>>(p, g, m, v, n, (float)(1.0 - lr * weight_decay), (float)(1.0 - beta1),
                                                 (float)beta2, (float)(1.0 - beta2), (float)sqrt(bc2), (float)eps,

@@ -1,6 +1,6 @@
 // Memory-bound kernels of the vision-tower backward pass ("next" row N1: the fine-tune step of reference
 // training/train_eval_loop.py:215-221 through HF CLIPVisionTransformer, i.e. what loss.backward() runs between the
-// GEMMs): dtype casts and transposes feeding the bf16 tcgen05 GEMMs, quick-GELU and LayerNorm backward, the softmax
+// GEMMs): dtype casts and transposes feeding the bf16 wgmma GEMMs, quick-GELU and LayerNorm backward, the softmax
 // correction term of attention backward, token-mean / embedding backward and bias gradients.  All HBM-bound:
 // vectorised, coalesced, grid-stride over the SMs.
 #include <cuda_bf16.h>
@@ -21,7 +21,7 @@ int check_launch(const char* what) {
   return 0;
 }
 
-inline int grid_1d(long work_items, int per_block, int cap = 148 * 16) {
+inline int grid_1d(long work_items, int per_block, int cap = 132 * 16) {
   long b = (work_items + per_block - 1) / per_block;
   if (b < 1) b = 1;
   return (int)(b > cap ? cap : b);
@@ -372,7 +372,7 @@ int layernorm_backward(const float* dy, const float* x, const float* gamma, floa
   if ((dgamma == nullptr) != (dbeta == nullptr)) { set_last_error("layernorm_backward: dgamma and dbeta go together"); return 1; }
   if (rows <= 0) return 0;
   long blocks = (rows + 7) / 8;
-  const long cap = (long)(num_sms > 0 ? num_sms : 148) * 8;
+  const long cap = (long)(num_sms > 0 ? num_sms : 132) * 8;
   if (blocks > cap) blocks = cap;
   ProfScope prof("train_ln_backward", stream);
   __nv_bfloat16* d16 = reinterpret_cast<__nv_bfloat16*>(dx_bf16);
@@ -393,7 +393,7 @@ int attention_delta(const float* d_out, const void* out_f16, float* delta, void*
   const long rows = (long)n_views * seq;
   if (rows <= 0) return 0;
   long blocks = (rows + 7) / 8;
-  const long cap = (long)(num_sms > 0 ? num_sms : 148) * 8;
+  const long cap = (long)(num_sms > 0 ? num_sms : 132) * 8;
   if (blocks > cap) blocks = cap;
   ProfScope prof("train_attention_delta", stream);
   PG_DISPATCH_NV4(hidden, (attention_delta_kernel<NV4><<<(int)blocks, 256, 0, stream>>>(

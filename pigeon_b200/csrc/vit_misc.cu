@@ -1,4 +1,4 @@
-// Memory-bound pieces of the CLIP vision tower around the tcgen05 GEMM / attention kernels:
+// Memory-bound pieces of the CLIP vision tower around the wgmma GEMM / attention kernels:
 // patch extraction (im2col), class-token + position embedding + pre_layrnorm, per-block LayerNorm,
 // and the token mean-pool that the reference applies to last_hidden_state
 // (models/clip_embedder.py:64-65, models/super_guessr.py:396-398).

@@ -62,8 +62,8 @@ int dgrad(const void* a, const void* w_t, float* out, long M, int N, int K, int 
 }
 
 // dw f32 [M, N] += left^T . right, with left [rows, M] and right [rows, N] row-major in any supported type.
-// Fast path: both operands as bf16 [rows, *] straight into the GEMM as MN-major UMMA operands (a cast where the saved
-// activation is fp16 — tcgen05 kind::f16 wants A and B of one type — and no transposes).  Otherwise (N % 256 != 0, the
+// Fast path: both operands as bf16 [rows, *] straight into the GEMM as MN-major wgmma operands (a cast where the saved
+// activation is fp16 — wgmma wants A and B of one type — and no transposes).  Otherwise (N % 256 != 0, the
 // patch embedding, or gathered rows): transpose both to bf16 [*, rows_p] and use the K-major kernel.
 int wgrad(const void* left, int left_type, long ld_left, int M, const void* right, int right_type, long ld_right, int N,
           long rows, float* dw, const BwdWs& w, int sms, cudaStream_t st, int map_div = 0, int map_mul = 0, int map_add = 0) {

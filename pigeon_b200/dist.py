@@ -3,7 +3,7 @@
 The reference's only inference-time collective is `accelerator.gather(output)` / `gather(index)` in
 preprocessing/embed.py:36-37 (torch.distributed all_gather via accelerate).  Here the per-rank head outputs
 (pooled embedding, top-k candidates, initial guess) are packed into one byte buffer and exchanged with a single
-`all_gather_into_tensor` (NCCL over NVLink on the B200 box; gloo in the CPU tests), issued on the compute stream.
+`all_gather_into_tensor` (NCCL over NVLink between the GPUs; gloo in the CPU tests), issued on the compute stream.
 """
 from __future__ import annotations
 

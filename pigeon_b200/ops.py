@@ -48,8 +48,8 @@ def attention_f16(qkv: torch.Tensor, n_views: int, seq: int, heads: int, variant
                   poly: int = -1, return_lse2: bool = False):
     """qkv fp16 [n_views*seq, 3*heads*64] -> fp16 [n_views*seq, heads*64].
 
-    `variant` (A/B measurements only): 0 = pair kernel, 1 = first-generation kernel, 2 = split kernel, 3 = fold kernel;
-    None = the library default.  `return_lse2` (with an explicit variant): also the log2-domain log-sum-exp of the scaled
+    `variant` (0..3) and `poly` are kept from earlier ABI versions that had several forward kernels; the sm_90a library
+    has one, and every value runs it.  None = pg_attention_f16.  `return_lse2` (with an explicit variant): also the log2-domain log-sum-exp of the scaled
     logits, f32 [n_views*heads, seq], the side output the training forward keeps for the backward pass."""
     _need_cuda(qkv)
     assert qkv.dtype == torch.float16 and qkv.shape == (n_views * seq, 3 * heads * 64)

@@ -1,4 +1,4 @@
-"""ProtoRefiner — prototype-retrieval guess refinement, B200 execution behind the reference's interface.
+"""ProtoRefiner — prototype-retrieval guess refinement, H100 execution behind the reference's interface.
 
 Mirror of reference models/proto_refiner.py: same constructor arguments and `forward(...)` keyword names and
 return value `(loss, preds_LLH, preds_geocell)`.  The per-query / per-candidate Python loops of the reference
@@ -41,7 +41,7 @@ class ProtoRefiner(nn.Module):
         super().__init__()
         if hedge:
             raise NotImplementedError("hedge=True (HedgeLayer, unused in the final model: models/README.md:11, "
-                                      "evaluate.py:73,79) is outside the B200 hot path")
+                                      "evaluate.py:73,79) is outside the H100 hot path")
         self.topk = topk
         self.hedge = hedge
         self.max_refinement = max_refinement

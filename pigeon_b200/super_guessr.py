@@ -1,8 +1,8 @@
-"""SuperGuessr — geocell classification model, B200 execution behind the reference's interface.
+"""SuperGuessr — geocell classification model, H100 execution behind the reference's interface.
 
 Mirror of reference models/super_guessr.py (same constructor arguments, `forward(...)` keyword names,
 `ModelOutput` / serving tuple, `load_state`, `lla_geocells`, `cell_layer`, `num_cells`).  The arithmetic
-of the inference branch (:386-466) and of the classification loss (:468-474) runs in the sm_100a kernels
+of the inference branch (:386-466) and of the classification loss (:468-474) runs in the sm_90a kernels
 of libpigeon_b200.so; there is no PyTorch/CPU fallback for it.
 """
 from __future__ import annotations
@@ -135,7 +135,7 @@ class CLIPVisionTower(nn.Module):
     def engine(self) -> VitEngine:
         p0 = next(self.parameters())
         if not p0.is_cuda:
-            raise PigeonB200Error("CLIPVisionTower is on the CPU: move the model with .to('cuda') — the B200 path "
+            raise PigeonB200Error("CLIPVisionTower is on the CPU: move the model with .to('cuda') — the H100 path "
                                   "has no CPU implementation")
         v = self._group_versions()
         if self._engine is None or self._packed_version != v:
@@ -185,9 +185,9 @@ class SuperGuessr(nn.Module):
             print(f'Not using keyword arguments: {list(kwargs.keys())}')  # :67-68
         if hierarchical:
             raise NotImplementedError("hierarchical=True (experimental self-attention pooling, disabled in the shipped "
-                                      "configs: evaluate.py:42, train_modes.py:99,126) is outside the B200 hot path")
+                                      "configs: evaluate.py:42, train_modes.py:99,126) is outside the H100 hot path")
         if heading and not panorama:
-            raise NotImplementedError("heading features for single images are outside the B200 hot path")
+            raise NotImplementedError("heading features for single images are outside the H100 hot path")
 
         self.base_model = as_tower(base_model)
         self.panorama = panorama
@@ -282,7 +282,7 @@ class SuperGuessr(nn.Module):
     def _device(self) -> torch.device:
         dev = self.cell_layer.weight.device
         if dev.type != 'cuda':
-            raise PigeonB200Error("SuperGuessr is on the CPU: call .to('cuda') — the B200 path has no CPU implementation")
+            raise PigeonB200Error("SuperGuessr is on the CPU: call .to('cuda') — the H100 path has no CPU implementation")
         return dev
 
     def _packed_head(self) -> Tensor:

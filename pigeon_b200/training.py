@@ -1,5 +1,5 @@
 """Fine-tune loop of the reference (training/train_eval_loop.py:164-253 `train_model`) for the part of the model the
-B200 path trains: the geocell head on embeddings (`on_embeddings=True`, base_model=None), the head on a frozen tower
+H100 path trains: the geocell head on embeddings (`on_embeddings=True`, base_model=None), the head on a frozen tower
 (`freeze_base=True`), and the tower itself under the reference's policy (super_guessr.py:159-160: embeddings frozen with all
 but the last encoder layer; `SuperGuessr._forward_train_tower` + `vit_train.TowerTrainer`).  Same loop shape — `output = model(**data)`, backward, gradient accumulation, AdamW step,
 evaluation and best-checkpoint saving per epoch — with `accelerate`/DDP replaced by torch.distributed plumbing

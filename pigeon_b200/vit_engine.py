@@ -57,7 +57,7 @@ def _strip_prefix(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
 
 
 class VitEngine:
-    """B200 execution engine of HF CLIPVisionTransformer.forward(...).last_hidden_state (+ token mean)."""
+    """H100 execution engine of HF CLIPVisionTransformer.forward(...).last_hidden_state (+ token mean)."""
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], dims: VitDims, device: torch.device | str = "cuda",
                  max_views_per_pass: int = 256, fold_layernorm: bool = True):

@@ -63,7 +63,7 @@ def evaluate(model: str, dataset, yfcc: bool, landmarks: bool = False, base_mode
 
 
 def main():
-    p = argparse.ArgumentParser(description='PIGEON hot path on B200 (embed / evaluate)')
+    p = argparse.ArgumentParser(description='PIGEON hot path on H100 (embed / evaluate)')
     p.add_argument('mode', choices=['pretrain', 'finetune', 'embed', 'evaluate'])
     p.add_argument('name', help='model / prediction-head path')
     p.add_argument('-l', '--load', default=None, help='comma-separated HF dataset directories')
@@ -76,7 +76,7 @@ def main():
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
     args = p.parse_args()
     if args.mode == 'pretrain':
-        raise NotImplementedError('"pretrain" (CLIP contrastive pre-training) is outside the B200 hot path')
+        raise NotImplementedError('"pretrain" (CLIP contrastive pre-training) is outside the H100 hot path')
     if args.load is None:
         raise NotImplementedError('A dataset must be given with -l (the reference regenerates it from un-shipped raw data).')
     from datasets import DatasetDict

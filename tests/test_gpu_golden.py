@@ -1,4 +1,4 @@
-"""Parity of the PUBLIC modules (pigeon_b200.SuperGuessr / CLIPEmbedding / ProtoRefiner -> C ABI -> sm_100a
+"""Parity of the PUBLIC modules (pigeon_b200.SuperGuessr / CLIPEmbedding / ProtoRefiner -> C ABI -> sm_90a
 kernels) against tests/golden/*.npz, i.e. against outputs of the UNMODIFIED reference modules on the same inputs.
 
 Tolerances: embeddings / logits-derived floats <= 1e-3 relative (BASELINE.json north_star); integer and index

@@ -1,4 +1,4 @@
-"""Kernel-level parity on the B200: each hand-written kernel against the same op in plain PyTorch fp32
+"""Kernel-level parity on the H100: each hand-written kernel against the same op in plain PyTorch fp32
 (a floating-point kernel's torch reference, evaluated on the SAME fp16-rounded operands so that the
 tolerance measures the kernel, not the quantisation)."""
 import math
@@ -52,7 +52,7 @@ def test_gemm_epilogues(cuda, M, N, K):
 
 
 def test_gemm_many_tiles_persistent(cuda):
-    """more tiles than SMs: exercises the persistent loop, both TMEM accumulator stages and the ring wrap."""
+    """more tiles than SMs: exercises the persistent loop, the reuse of the accumulator tile and the ring wrap."""
     from pigeon_b200 import _lib, ops
     g = torch.Generator(device="cpu").manual_seed(5)
     M, N, K = 577 * 64, 1024, 1024
@@ -97,7 +97,7 @@ def test_attention(cuda, n_views, seq, heads):
     assert torch.isfinite(out.float()).all()
 
 
-ATTN_KERNELS = [(None, -1), (3, 2), (3, 12), (0, 2), (2, 2), (1, 0)]   # default, fold, fold with two threads per row, pair, split, first
+ATTN_KERNELS = [(None, -1), (3, 2), (3, 12), (0, 2), (2, 2), (1, 0)]   # default entry point, then every (variant, poly) the ABI accepts
 
 
 def _attention_reference(qkv, n_views, seq, heads):
@@ -108,10 +108,23 @@ def _attention_reference(qkv, n_views, seq, heads):
     return out, logits
 
 
+def test_attention_views_are_independent(cuda):
+    """A view's last KV block ends inside the next view's rows: non-finite values there must not reach this view."""
+    from pigeon_b200 import ops
+    n_views, seq, heads = 2, 65, 2
+    g = torch.Generator(device="cpu").manual_seed(5)
+    qkv = (torch.randn(n_views * seq, 3 * heads * 64, generator=g) * 1.5).half()
+    ref, _ = _attention_reference(qkv[:seq].to(cuda), 1, seq, heads)
+    qkv[seq:] = float("nan")
+    out = ops.attention_f16(qkv.to(cuda), n_views, seq, heads)
+    assert torch.isfinite(out[:seq].float()).all()
+    assert _rel(out[:seq].float(), ref) < 2e-3
+
+
 @pytest.mark.parametrize("variant,poly", ATTN_KERNELS[1:])
 @pytest.mark.parametrize("n_views,seq,heads", [(2, 577, 3), (1, 17, 4), (3, 200, 1), (2, 64, 2), (1, 129, 5)])
 def test_attention_every_kernel_and_its_lse2(cuda, n_views, seq, heads, variant, poly):
-    """Every forward kernel generation against torch fp32, output and the log2-domain log-sum-exp side output (what the
+    """Every (variant, poly) of the ABI against torch fp32, output and the log2-domain log-sum-exp side output (what the
     training forward keeps for the backward)."""
     from pigeon_b200 import ops
     g = torch.Generator(device="cpu").manual_seed(seq * 5 + heads)
@@ -126,8 +139,7 @@ def test_attention_every_kernel_and_its_lse2(cuda, n_views, seq, heads, variant,
 @pytest.mark.parametrize("variant,poly", ATTN_KERNELS)
 def test_attention_growing_logits_exercise_rescale(cuda, variant, poly):
     """Key norms grow along the sequence so that later KV blocks raise the row maximum far beyond what fp16 P can hold
-    relative to the first block: the pair / first-generation kernels must rescale O and l in TMEM, the fold kernel must take
-    its exact per-row repair path — all must agree with an exact softmax."""
+    relative to the first block: the kernel must rescale O and l when the maximum rises and agree with an exact softmax."""
     from pigeon_b200 import ops
     n_views, seq, heads = 2, 577, 2
     g = torch.Generator(device="cpu").manual_seed(77)
@@ -143,7 +155,7 @@ def test_attention_growing_logits_exercise_rescale(cuda, variant, poly):
     assert (spread < 18).float().mean() > 0.2, "and leave others inside it"
     err = _rel(out.float(), ref)
     assert torch.isfinite(out.float()).all() and err < 2e-3, err
-    # row by row: the repaired rows and the fast-path rows are both right
+    # row by row: the rescaled rows and the others are both right
     row_err = (out.float() - ref).norm(dim=1) / ref.norm(dim=1).clamp_min(1e-6)
     assert row_err.max().item() < 2e-2, row_err.max().item()
 

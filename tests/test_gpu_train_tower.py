@@ -189,7 +189,7 @@ def test_tower_backward_matches_reference_autograd(cuda, name):
     np.testing.assert_allclose(float(out.loss), float(z["loss"]), rtol=1e-3)
     sg.backward(out.loss)
     worst = _check_grads(sg, z, meta)
-    try:                                   # measured parity, picked up into profiles/ by hand; never fails the test
+    try:                                   # measured parity, appended to a log; never fails the test
         d = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
         os.makedirs(d, exist_ok=True)
         with open(os.path.join(d, "parity.log"), "a") as f:

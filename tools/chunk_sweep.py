@@ -1,4 +1,4 @@
-"""Tower throughput vs views per pass (workspace chunk): smaller chunks keep more of the activations in the 126 MB L2
+"""Tower throughput vs views per pass (workspace chunk): smaller chunks keep more of the activations in the 50 MB L2
 at the price of fewer tiles per GEMM launch.  Same weights and pixels for every setting, alternating, CUDA events."""
 import json
 import os
