@@ -88,6 +88,63 @@ size_t pg_vit_workspace_bytes(const pg_vit* h, int32_t n_views);
  *   -> hidden_out (optional, may be NULL) f32 [n_views, tokens, hidden] = last_hidden_state. */
 int pg_vit_forward(pg_vit* h, const void* pixels, int32_t pixels_f16, int32_t n_views, void* workspace,
                    size_t workspace_bytes, float* emb_out, float* hidden_out, void* stream);
+/* pg_vit_forward plus cls_out f32 [n_views, hidden] = last_hidden_state[:, 0], the CLS rows that HF
+ * CLIPVisionTransformer pools into post_layernorm (transformers 4.23.1 modeling_clip.py, `pooled_output =
+ * last_hidden_state[:, 0, :]`) and CLIPModel.get_image_features projects — without writing the whole hidden_out.
+ * hidden_out may still be given (or NULL). */
+int pg_vit_forward_cls(pg_vit* h, const void* pixels, int32_t pixels_f16, int32_t n_views, void* workspace,
+                       size_t workspace_bytes, float* emb_out, float* hidden_out, float* cls_out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
+ * CLIP text tower and image-text logits (HF CLIPModel, transformers 4.23.1 modeling_clip.py, the dual encoder that
+ * reference training/train_modes.py:30-64 pretrains and dataset_creation/pretrain/pretrain_dataset.py:299-330 scores:
+ * `model(**clip_processor(text=captions, images=images), return_loss=True).logits_per_image.softmax(1).argmax(1)`).
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct pg_text_config {
+  int32_t vocab;          /* 49408 */
+  int32_t max_positions;  /* 77 */
+  int32_t hidden;         /* 768, multiple of 256 */
+  int32_t heads;          /* 12, hidden / heads must be 64 */
+  int32_t intermediate;   /* 3072, multiple of 256 */
+  int32_t layers;         /* 12 */
+  float ln_eps;           /* 1e-5 */
+} pg_text_config;
+
+/* HF CLIPTextTransformer weights.  The encoder layers are the vision tower's pg_vit_layer (same pre-LN CLIPEncoderLayer)
+ * with the LayerNorm-fold fields NULL: the text tower runs the LayerNorm kernels. */
+typedef struct pg_text_weights {
+  const float* token_emb;        /* f32 [vocab, hidden]          embeddings.token_embedding.weight */
+  const float* pos_emb;          /* f32 [max_positions, hidden]  embeddings.position_embedding.weight */
+  const pg_vit_layer* layers_host;  /* HOST array of `layers` entries (device pointers inside) */
+  const float* final_ln_g; const float* final_ln_b;   /* final_layer_norm [hidden] */
+} pg_text_weights;
+
+typedef struct pg_text pg_text;
+
+int pg_text_create(const pg_text_config* cfg, const pg_text_weights* w, pg_text** out);
+void pg_text_destroy(pg_text* h);
+/* Scratch needed by pg_text_forward for n captions of S tokens. */
+size_t pg_text_workspace_bytes(const pg_text* h, int32_t n, int32_t S);
+/* HF CLIPTextTransformer.forward (4.23.1): input_ids i64 [n, S] (1 <= S <= max_positions), attention_mask i64 [n, S] or
+ * NULL (all ones; 0 excludes that key, on top of the causal mask; attention_mask[:, 0] must be 1, as CLIP's BOS is)
+ *   -> pooled_out f32 [n, hidden] = final_layer_norm(x)[b, argmax_t input_ids[b, t]] (first index of the largest id);
+ *   -> hidden_out (optional) f32 [n, S, hidden] = last_hidden_state (after final_layer_norm). */
+int pg_text_forward(pg_text* h, const int64_t* input_ids, const int64_t* attention_mask, int32_t n, int32_t S,
+                    void* workspace, size_t workspace_bytes, float* pooled_out, float* hidden_out, void* stream);
+
+/* visual_projection / text_projection (nn.Linear, no bias) at fp32-faithful accuracy: x f32 [n, D], optional LayerNorm
+ * (ln_g and ln_b both NULL = none; CLIPModel.get_image_features applies post_layernorm here), then the error-compensated
+ * split GEMM of the geocell head: w3 = pg_head_pack_weight(W f32 [P, D]) fp16 [P, 3 D]  ->  out f32 [n, P] = LN(x) W^T. */
+size_t pg_clip_project_workspace_bytes(int32_t n, int32_t D);
+int pg_clip_project(const float* x, int32_t n, int32_t D, const float* ln_g, const float* ln_b, float ln_eps, const void* w3,
+                    int32_t P, void* workspace, size_t workspace_bytes, float* out, void* stream);
+/* CLIPModel.forward after the projections: img f32 [Ni, P], txt f32 [Nt, P] (not normalised)
+ *   -> logits_per_image f32 [Ni, Nt] = (img / |img|) (txt / |txt|)^T * exp(logit_scale);
+ *   -> optional (NULL = not written): logits_per_text f32 [Nt, Ni] (the transpose), probs f32 [Ni, Nt] (softmax over the
+ *      captions), pred i64 [Ni] (first argmax), loss f32 [1] = clip_loss (mean of the two cross-entropies against arange;
+ *      needs Ni == Nt). */
+int pg_clip_logits(const float* img, int32_t Ni, const float* txt, int32_t Nt, int32_t P, float logit_scale,
+                   float* logits_per_image, float* logits_per_text, float* probs, int64_t* pred, float* loss, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Geocell head (reference models/super_guessr.py:437-459: view mean, cell_layer, softmax, argmax, top-k)
@@ -330,6 +387,11 @@ int pg_layernorm_f16(const float* x, void* y, const float* gamma, const float* b
                      float eps, void* stream);
 /* softmax(q k^T / 8) v per (view, head); qkv fp16 [n_views*seq, 3*heads*64] -> out fp16 [n_views*seq, heads*64]. */
 int pg_attention_f16(const void* qkv, void* out, int32_t n_views, int32_t seq, int32_t heads, void* stream);
+/* The text tower's attention (HF CLIPTextTransformer: causal mask + expanded attention_mask, 4.23.1): key j is admissible
+ * for query i only if (causal == 0 or j <= i) and (mask == NULL or mask[view, j] != 0); mask i64 [n_views, seq],
+ * mask[:, 0] must be non-zero.  mask NULL and causal 0 is pg_attention_f16, bit for bit. */
+int pg_attention_f16_masked(const void* qkv, void* out, const int64_t* mask, int32_t causal, int32_t n_views, int32_t seq,
+                            int32_t heads, void* stream);
 /* The same op with the optional lse2 side output (may be NULL).  `variant` (0..3) and `poly` selected among several forward
  * kernels in earlier versions of this ABI; the sm_90a library has one wgmma kernel, and every variant runs it. */
 int pg_attention_f16_variant(const void* qkv, void* out, float* lse2, int32_t n_views, int32_t seq, int32_t heads,

@@ -5,6 +5,8 @@
     ProtoRefiner   (reference models/proto_refiner.py)   prototype retrieval refinement
     train_model, AdamW (reference training/train_eval_loop.py:164-253)   fine-tune step: head and tower backward
     ClipImageProcessor (the reference's CLIPProcessor call sites)        image pre-processing on the GPU
+    CLIPModel, CLIPTextTower (HF CLIPModel as training/train_modes.py:30-64 uses it)   text tower + image-text logits
+    get_caption_probabilities, zero_shot_accuracy (names evaluation/__init__.py:3 imports)   zero-shot caption scoring
 
 Host code is Python/PyTorch plumbing over a C-ABI CUDA library (include/pigeon_b200.h); see DESIGN.md.
 """
@@ -26,6 +28,15 @@ def __getattr__(name):  # lazy: these import pandas / transformers-sized depende
     if name in ("train_model", "AdamW", "finetune_model", "finetune_on_embeddings"):
         from . import training
         return getattr(training, name)
+    if name in ("CLIPTextTower", "TextDims", "TextEngine"):
+        from . import clip_text
+        return getattr(clip_text, name)
+    if name in ("CLIPModel", "CLIPOutput"):
+        from . import clip_model
+        return getattr(clip_model, name)
+    if name in ("get_caption_probabilities", "zero_shot_accuracy"):
+        from . import zeroshot
+        return getattr(zeroshot, name)
     if name == "ClipImageProcessor":
         from .preprocess import ClipImageProcessor
         return ClipImageProcessor

@@ -34,6 +34,8 @@ SOURCES = [
     "attention_bwd_wgmma.cu",
     "vit_train_capi.cu",
     "capi.cu",
+    "clip.cu",
+    "clip_capi.cu",
 ]
 
 NVCC_FLAGS = [

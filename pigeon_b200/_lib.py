@@ -58,6 +58,16 @@ class VitWeights(C.Structure):
                 ("pre_ln_b", c_void_p), ("layers_host", C.POINTER(VitLayer))]
 
 
+class TextConfig(C.Structure):
+    _fields_ = [("vocab", c_int32), ("max_positions", c_int32), ("hidden", c_int32), ("heads", c_int32),
+                ("intermediate", c_int32), ("layers", c_int32), ("ln_eps", c_float)]
+
+
+class TextWeights(C.Structure):
+    _fields_ = [("token_emb", c_void_p), ("pos_emb", c_void_p), ("layers_host", C.POINTER(VitLayer)),
+                ("final_ln_g", c_void_p), ("final_ln_b", c_void_p)]
+
+
 class RefinerBank(C.Structure):
     _fields_ = [("num_cells", c_int32), ("dim", c_int32), ("cell_off", c_void_p), ("proto_emb", c_void_p),
                 ("proto_lnglat", c_void_p), ("proto_count", c_void_p), ("member_off", c_void_p),
@@ -73,6 +83,18 @@ SIGNATURES = {
     "pg_vit_destroy": (None, [c_void_p]),
     "pg_vit_workspace_bytes": (c_size_t, [c_void_p, c_int32]),
     "pg_vit_forward": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+    "pg_vit_forward_cls": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p,
+                                     c_void_p]),
+    "pg_text_create": (c_int32, [C.POINTER(TextConfig), C.POINTER(TextWeights), C.POINTER(c_void_p)]),
+    "pg_text_destroy": (None, [c_void_p]),
+    "pg_text_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
+    "pg_text_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_size_t, c_void_p, c_void_p,
+                                  c_void_p]),
+    "pg_clip_project_workspace_bytes": (c_size_t, [c_int32, c_int32]),
+    "pg_clip_project": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_float, c_void_p, c_int32, c_void_p,
+                                  c_size_t, c_void_p, c_void_p]),
+    "pg_clip_logits": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_float, c_void_p, c_void_p, c_void_p,
+                                 c_void_p, c_void_p, c_void_p]),
     "pg_vit_forward_train": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, C.POINTER(VitSaved), c_void_p, c_void_p]),
     "pg_vit_backward_workspace_bytes": (c_size_t, [c_void_p, c_int32]),
     "pg_vit_backward": (c_int32, [c_void_p, C.POINTER(VitSaved), c_void_p, c_int32, C.POINTER(VitGrads), c_void_p, c_size_t,
@@ -128,6 +150,7 @@ SIGNATURES = {
                               c_int32, c_int32, c_void_p]),
     "pg_layernorm_f16": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_float, c_void_p]),
     "pg_attention_f16": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
+    "pg_attention_f16_masked": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "pg_attention_f16_variant": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32,
                                            c_void_p]),
 }

@@ -1,0 +1,143 @@
+"""CLIPModel — HF `CLIPModel`'s forward (transformers 4.23.1 modeling_clip.py) on the GPU: the dual encoder that reference
+training/train_modes.py:30-64 pretrains into StreetCLIP and that `PretrainDataset.accuracy`
+(dataset_creation/pretrain/pretrain_dataset.py:299-330, pretrain_dataset_yfcc.py:220-246) scores with
+`model(**clip_processor(text=captions, images=images), return_loss=True).logits_per_image.softmax(1).argmax(1)`.
+
+Parameter names are HF's (`text_model.*`, `vision_model.*`, `visual_projection.weight`, `text_projection.weight`,
+`logit_scale`), so CLIPModel checkpoints load by name.  Forward only: the pretraining step is not implemented.
+
+    image features = visual_projection(post_layernorm(last_hidden_state[:, 0]))      (CLS row; pg_vit_forward_cls)
+    text features  = text_projection(pooled)                                          (pg_text_forward)
+    logits_per_text = normalise(text) @ normalise(image)^T * exp(logit_scale), logits_per_image = its transpose,
+    loss = mean of the two cross-entropies against arange                             (pg_clip_logits)
+The projections run the geocell head's error-compensated fp16 split GEMM (fp32-faithful, pg_clip_project).
+"""
+from __future__ import annotations
+
+import math
+from dataclasses import dataclass
+from typing import Optional
+
+import torch
+from torch import Tensor, nn
+from torch.nn.parameter import Parameter
+
+from . import _versions, ops
+from ._lib import PigeonB200Error
+from .clip_text import CLIPTextTower, TextDims, _Holder, check_sequence_length
+from .super_guessr import CLIPVisionTower
+from .vit_engine import VitDims
+
+LOGIT_SCALE_INIT = math.log(1 / 0.07)   # CLIPConfig.logit_scale_init_value (2.6592)
+
+
+@dataclass
+class CLIPOutput:
+    """The fields of HF `CLIPOutput` that the forward computes (text_embeds / image_embeds are L2-normalised, as HF's)."""
+    loss: Optional[Tensor] = None
+    logits_per_image: Optional[Tensor] = None
+    logits_per_text: Optional[Tensor] = None
+    text_embeds: Optional[Tensor] = None
+    image_embeds: Optional[Tensor] = None
+
+    def __getitem__(self, key):
+        return getattr(self, key)
+
+
+class CLIPModel(nn.Module):
+    def __init__(self, text_dims: TextDims = TextDims(), vision_dims: VitDims = VitDims(), projection_dim: int = 768):
+        super().__init__()
+        self.text_dims, self.vision_dims, self.projection_dim = text_dims, vision_dims, projection_dim
+        # The towers own the kernels; their parameter trees are registered here under HF's names.
+        self._towers = (CLIPTextTower(text_dims), CLIPVisionTower(vision_dims))
+        self.text_model = self._towers[0].text_model
+        self.vision_model = self._towers[1].vision_model
+        self.visual_projection = _Holder()
+        self.visual_projection.weight = Parameter(torch.zeros(projection_dim, vision_dims.hidden))
+        self.text_projection = _Holder()
+        self.text_projection.weight = Parameter(torch.zeros(projection_dim, text_dims.hidden))
+        self.logit_scale = Parameter(torch.tensor(LOGIT_SCALE_INIT))
+        self._packed = {}
+
+    @property
+    def text_tower(self) -> CLIPTextTower:
+        return self._towers[0]
+
+    @property
+    def vision_tower(self) -> CLIPVisionTower:
+        return self._towers[1]
+
+    def _apply(self, fn, *args, **kwargs):
+        # .to() / .cuda() move the shared parameters; the towers' engines repack from them lazily
+        super()._apply(fn, *args, **kwargs)
+        for t in self._towers:
+            t._engine, t._packed_version = None, None
+        self._packed = {}
+        return self
+
+    @classmethod
+    def from_hf(cls, hf_model) -> "CLIPModel":
+        """Build from a HuggingFace CLIPModel instance (weights copied by name)."""
+        cfg = hf_model.config
+        model = cls(TextDims.from_hf_config(cfg.text_config), VitDims.from_hf_config(cfg.vision_config),
+                    projection_dim=cfg.projection_dim)
+        sd = {k: v for k, v in hf_model.state_dict().items() if "position_ids" not in k}
+        missing, unexpected = model.load_state_dict(sd, strict=False)
+        if missing or unexpected:
+            raise PigeonB200Error(f"cannot map HF weights: missing={missing} unexpected={unexpected}")
+        return model
+
+    # ------------------------------------------------------------------------------------------ kernels
+    def _packed_projection(self, name: str) -> Tensor:
+        w = getattr(self, name).weight
+        key = (w.data_ptr(), w._version, _versions.get(w))
+        hit = self._packed.get(name)
+        if hit is None or hit[0] != key:
+            hit = (key, ops.head_pack_weight(w.detach()))
+            self._packed[name] = hit
+        return hit[1]
+
+    def _check_cuda(self):
+        if not self.logit_scale.is_cuda:
+            raise PigeonB200Error("CLIPModel is on the CPU: move the model with .to('cuda') — the H100 path has no CPU "
+                                  "implementation")
+
+    @torch.no_grad()
+    def get_text_features(self, input_ids: Tensor, attention_mask: Optional[Tensor] = None) -> Tensor:
+        """text_projection(pooler_output) f32 [n, projection_dim] (not normalised, as HF's)."""
+        self._check_cuda()
+        pooled = self.text_tower.pooled(input_ids, attention_mask)
+        return ops.clip_project(pooled, self._packed_projection("text_projection"))
+
+    @torch.no_grad()
+    def get_image_features(self, pixel_values: Tensor) -> Tensor:
+        """visual_projection(post_layernorm(last_hidden_state[:, 0])) f32 [n, projection_dim] (not normalised, as HF's)."""
+        self._check_cuda()
+        _, cls = self.vision_tower.engine().forward_cls(pixel_values)
+        post = self.vision_model.post_layernorm
+        return ops.clip_project(cls, self._packed_projection("visual_projection"), post.weight.detach(),
+                                post.bias.detach(), self.vision_dims.ln_eps)
+
+    def logits(self, image_features: Tensor, text_features: Tensor, **want) -> dict:
+        """`ops.clip_logits` at this model's logit_scale (features need not be normalised)."""
+        return ops.clip_logits(image_features, text_features, float(self.logit_scale.detach()), **want)
+
+    @torch.no_grad()
+    def forward(self, input_ids: Tensor = None, pixel_values: Tensor = None, attention_mask: Tensor = None,
+                return_loss: bool = False) -> CLIPOutput:
+        """HF CLIPModel.forward: the reference's `model(**inputs)` with inputs from `CLIPProcessor(text=..., images=...)`
+        (input_ids, attention_mask, pixel_values) and `return_loss=True`."""
+        if input_ids is None or pixel_values is None:
+            raise ValueError("CLIPModel.forward needs both input_ids and pixel_values")
+        check_sequence_length(input_ids.shape[-1], self.text_dims.max_positions)
+        if return_loss and input_ids.shape[0] != pixel_values.shape[0]:
+            raise ValueError(f"the contrastive loss needs as many images as captions (got {pixel_values.shape[0]} images, "
+                             f"{input_ids.shape[0]} captions)")
+        image_features = self.get_image_features(pixel_values)
+        text_features = self.get_text_features(input_ids, attention_mask)
+        out = self.logits(image_features, text_features, per_text=True, loss=bool(return_loss))
+        # HF returns the normalised embeds; the logits above normalise inside the kernel
+        return CLIPOutput(loss=out.get("loss"), logits_per_image=out["logits_per_image"],
+                          logits_per_text=out["logits_per_text"],
+                          text_embeds=text_features / text_features.norm(p=2, dim=-1, keepdim=True),
+                          image_embeds=image_features / image_features.norm(p=2, dim=-1, keepdim=True))

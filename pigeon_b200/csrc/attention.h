@@ -8,6 +8,10 @@ namespace pg {
 // lse2 (optional): f32 [n_views*heads, seq], log2-domain log-sum-exp of the scaled logits, kept for the backward pass.
 int attention_f16(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream,
                   float* lse2 = nullptr);
+// The text tower's variant: causal (key j admissible for query i only if j <= i) and / or a key mask i64 [n_views, seq]
+// (0 = excluded).  mask == nullptr and causal == 0 runs attention_f16 itself.  mask[v, 0] must be non-zero.
+int attention_f16_masked(const void* qkv, void* out, const long long* mask, int causal, int n_views, int seq, int heads,
+                         cudaStream_t stream);
 
 // Backward of the attention core (attention_bwd_wgmma.cu).
 //   qkv f16 / qkv_bf16 [n_views*seq, 3*heads*64] (same values, two operand types), d_out_bf16 [n_views*seq, heads*64],

@@ -18,6 +18,12 @@
 //                            the accumulator fragment of S is exactly the A-operand fragment of the next MMA;
 //   O += P_j V_j             wgmma with A from registers and V as an MN-major shared-memory operand.
 // Final O / l -> fp16 through shared memory (16-byte coalesced stores).
+//
+// kMasked = true is the text tower's variant (HF CLIPTextTransformer: causal mask plus the padding `attention_mask`,
+// modeling_clip.py 4.23.1 `_build_causal_attention_mask` / `_expand_mask`): key j is admissible for query i only if
+// j <= i (causal) and mask[view, j] != 0, applied on the S fragment where the ragged-tail test sits.  A causal q-tile stops
+// at its diagonal KV block.  Block 0 holds key 0, which every row admits as long as mask[view, 0] != 0 (CLIP's BOS):
+// the running maximum is then finite after the first block and the rescale ex2((m - n) c) never sees -inf - -inf.
 #include "attention.h"
 #include "prof.h"
 #include "ptx.cuh"
@@ -43,6 +49,8 @@ struct AttnArgs {
   __half* out;  // [n_views*seq, hidden]
   float scale_log2;  // (1/sqrt(64)) * log2(e)
   float* lse2;       // optional [n_views * heads, seq]: log2-domain log-sum-exp of the scaled logits (for the backward pass)
+  const long long* mask;   // kMasked: optional [n_views, seq], 0 = key excluded
+  int causal;              // kMasked: key j admissible for query i only if j <= i
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -51,6 +59,7 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
+template <bool kMasked>
 __global__ void __launch_bounds__(kThreads, 4)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnArgs args) {
   extern __shared__ uint8_t smem_raw[];
@@ -65,7 +74,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnArgs ar
   const int lane = threadIdx.x & 31;
   const int q_tile = blockIdx.x, head = blockIdx.y, view = blockIdx.z;
   const int S = args.seq;
-  const int nb = (S + kBlockKV - 1) / kBlockKV;                 // KV blocks (10 for S = 577)
+  int nb = (S + kBlockKV - 1) / kBlockKV;                       // KV blocks (10 for S = 577)
+  if constexpr (kMasked) {
+    if (args.causal && q_tile + 1 < nb) nb = q_tile + 1;        // kBlockQ == kBlockKV: the diagonal block is q_tile
+  }
   const int row0 = view * S;                                    // first row of this view in qkv / out
   const int q_col = head * kHeadDim, k_col = args.hidden + q_col, v_col = 2 * args.hidden + q_col;
 
@@ -115,12 +127,26 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnArgs ar
 
     // kv columns past the view (last block only) drop out of the maximum and get P = 0; their K / V rows are zeros (the
     // tensor map is per view, so TMA zero-fills past the last token and no other view's data enters this one's MMAs)
-    const int valid = S - j * kBlockKV;
-    if (valid < kBlockKV) {
+    if constexpr (kMasked) {
+      // rows 16 warp + lane / 4 (s[4g], s[4g + 1]) and that + 8 (s[4g + 2], s[4g + 3]) of the q-tile
+      const int q0 = q_tile * kBlockQ + 16 * warp + (lane >> 2);
+      const long long* mrow = args.mask ? args.mask + (size_t)view * S : nullptr;
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
-        const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-        if (col >= valid) s[i] = -INFINITY;
+        const int kv = j * kBlockKV + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        bool ok = kv < S;
+        if (args.causal) ok = ok && kv <= q0 + 8 * ((i >> 1) & 1);
+        if (mrow) ok = ok && __ldg(mrow + kv) != 0;
+        if (!ok) s[i] = -INFINITY;
+      }
+    } else {
+      const int valid = S - j * kBlockKV;
+      if (valid < kBlockKV) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+          if (col >= valid) s[i] = -INFINITY;
+        }
       }
     }
     float b0 = -INFINITY, b1 = -INFINITY;
@@ -193,20 +219,20 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnArgs ar
   }
 }
 
-}  // namespace
-
-int attention_f16(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream, float* lse2) {
+template <bool kMasked>
+int launch_attention(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream, float* lse2,
+                     const long long* mask, int causal, const char* name) {
   if (n_views <= 0) return 0;
   if (n_views > 65535) { set_last_error("attention: n_views %d > 65535 (grid.z)", n_views); return 1; }
   const int hidden = heads * kHeadDim;
   CUtensorMap tm;
   if (make_tmap_f16_3d(&tm, qkv, n_views, seq, 3 * hidden, 3 * hidden, kBlockKV, kHeadDim)) return 1;
-  static std::atomic<int> attr_set_dev[64];   // per device (the attribute is per context)
+  static std::atomic<int> attr_set_dev[64];   // per instantiation and device (the attribute is per context)
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64) dev = 0;
   if (!attr_set_dev[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(attention_kernel<kMasked>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
     if (e != cudaSuccess) { set_last_error("attention: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return 1; }
     attr_set_dev[dev].store(1, std::memory_order_release);
   }
@@ -216,12 +242,26 @@ int attention_f16(const void* qkv, void* out, int n_views, int seq, int heads, c
   a.out = reinterpret_cast<__half*>(out);
   a.scale_log2 = 0.125f * 1.4426950408889634f;
   a.lse2 = lse2;
+  a.mask = mask;
+  a.causal = causal;
   dim3 grid((seq + kBlockQ - 1) / kBlockQ, heads, n_views);
-  ProfScope prof("attention", stream);
-  attention_kernel<<<grid, kThreads, kSmemBytes, stream>>>(tm, a);
+  ProfScope prof(name, stream);
+  attention_kernel<kMasked><<<grid, kThreads, kSmemBytes, stream>>>(tm, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error("attention launch: %s", cudaGetErrorString(e)); return 1; }
   return 0;
+}
+
+}  // namespace
+
+int attention_f16(const void* qkv, void* out, int n_views, int seq, int heads, cudaStream_t stream, float* lse2) {
+  return launch_attention<false>(qkv, out, n_views, seq, heads, stream, lse2, nullptr, 0, "attention");
+}
+
+int attention_f16_masked(const void* qkv, void* out, const long long* mask, int causal, int n_views, int seq, int heads,
+                         cudaStream_t stream) {
+  if (!mask && !causal) return attention_f16(qkv, out, n_views, seq, heads, stream);
+  return launch_attention<true>(qkv, out, n_views, seq, heads, stream, nullptr, mask, causal ? 1 : 0, "attention_masked");
 }
 
 }  // namespace pg

@@ -39,6 +39,42 @@ int sm_count() {
   return g_sm_count;
 }
 
+// Pre-LN CLIPEncoderLayer stack with the LayerNorm kernels (HF modeling_clip.py 4.23.1 CLIPEncoderLayer.forward):
+//   x += out_proj(attn(layer_norm1(x)));  x += fc2(quick_gelu(fc1(layer_norm2(x))))
+// on x f32 [n_seq * seq, hidden]; xn / u are the fp16 scratch of vit_carve.  The vision tower passes mask = NULL and
+// causal = 0 (plain attention_f16); the text tower its attention_mask and causal = 1.
+int encoder_layers(const pg_vit_layer* layers, int n_layers, int hidden, int heads, int intermediate, float eps, float* x,
+                   void* xn, void* u, int n_seq, int seq, const int64_t* mask, int causal, int sms, cudaStream_t stream) {
+  const long rows = (long)n_seq * seq;
+  for (int l = 0; l < n_layers; ++l) {
+    const pg_vit_layer& L = layers[l];
+    if (layernorm_f16(x, xn, L.ln1_g, L.ln1_b, rows, hidden, eps, sms, stream)) return 1;
+    GemmProblem p{};
+    p.M = (int)rows; p.N = 3 * hidden; p.K = hidden;
+    p.a = xn; p.lda = hidden; p.w = L.w_qkv; p.ldw = hidden;
+    p.out = u; p.ldo = 3 * hidden; p.bias = L.b_qkv; p.epi = EPI_F16_BIAS;
+    if (gemm_f16(p, sms, stream)) return 1;
+    if (attention_f16_masked(u, xn, reinterpret_cast<const long long*>(mask), causal, n_seq, seq, heads, stream)) return 1;
+    p = GemmProblem{};
+    p.M = (int)rows; p.N = hidden; p.K = hidden;
+    p.a = xn; p.lda = hidden; p.w = L.w_o; p.ldw = hidden;
+    p.out = x; p.ldo = hidden; p.bias = L.b_o; p.epi = EPI_F32_BIAS_RESID;
+    if (gemm_f16(p, sms, stream)) return 1;
+    if (layernorm_f16(x, xn, L.ln2_g, L.ln2_b, rows, hidden, eps, sms, stream)) return 1;
+    p = GemmProblem{};
+    p.M = (int)rows; p.N = intermediate; p.K = hidden;
+    p.a = xn; p.lda = hidden; p.w = L.w_fc1; p.ldw = hidden;
+    p.out = u; p.ldo = intermediate; p.bias = L.b_fc1; p.epi = EPI_F16_BIAS_QGELU;
+    if (gemm_f16(p, sms, stream)) return 1;
+    p = GemmProblem{};
+    p.M = (int)rows; p.N = hidden; p.K = intermediate;
+    p.a = u; p.lda = intermediate; p.w = L.w_fc2; p.ldw = intermediate;
+    p.out = x; p.ldo = hidden; p.bias = L.b_fc2; p.epi = EPI_F32_BIAS_RESID;
+    if (gemm_f16(p, sms, stream)) return 1;
+  }
+  return 0;
+}
+
 }  // namespace pg
 
 extern "C" {
@@ -101,8 +137,8 @@ size_t pg_vit_workspace_bytes(const pg_vit* h, int32_t n_views) {
   return vit_carve(h, n_views, nullptr, &x, &xn, &u);
 }
 
-int pg_vit_forward(pg_vit* h, const void* pixels, int32_t pixels_f16, int32_t n_views, void* workspace,
-                   size_t workspace_bytes, float* emb_out, float* hidden_out, void* stream_) {
+static int vit_forward(pg_vit* h, const void* pixels, int32_t pixels_f16, int32_t n_views, void* workspace,
+                       size_t workspace_bytes, float* emb_out, float* hidden_out, float* cls_out, void* stream_) {
   if (!h || !pixels || !workspace || !emb_out) { set_last_error("pg_vit_forward: null argument"); return 1; }
   if (n_views <= 0) return 0;
   const int sms = sm_count();
@@ -163,38 +199,32 @@ int pg_vit_forward(pg_vit* h, const void* pixels, int32_t pixels_f16, int32_t n_
     if (gemm_f16(p, sms, stream)) return 1;
   }
 
-  for (int l = 0; !folded && l < c.layers; ++l) {
-    const pg_vit_layer& L = h->layers[l];
-    if (layernorm_f16(x, xn, L.ln1_g, L.ln1_b, rows, c.hidden, c.ln_eps, sms, stream)) return 1;
-    GemmProblem p{};
-    p.M = (int)rows; p.N = 3 * c.hidden; p.K = c.hidden;
-    p.a = xn; p.lda = c.hidden; p.w = L.w_qkv; p.ldw = c.hidden;
-    p.out = u; p.ldo = 3 * c.hidden; p.bias = L.b_qkv; p.epi = EPI_F16_BIAS;
-    if (gemm_f16(p, sms, stream)) return 1;
-    if (attention_f16(u, xn, n_views, h->tokens, c.heads, stream)) return 1;
-    p = GemmProblem{};
-    p.M = (int)rows; p.N = c.hidden; p.K = c.hidden;
-    p.a = xn; p.lda = c.hidden; p.w = L.w_o; p.ldw = c.hidden;
-    p.out = x; p.ldo = c.hidden; p.bias = L.b_o; p.epi = EPI_F32_BIAS_RESID;
-    if (gemm_f16(p, sms, stream)) return 1;
-    if (layernorm_f16(x, xn, L.ln2_g, L.ln2_b, rows, c.hidden, c.ln_eps, sms, stream)) return 1;
-    p = GemmProblem{};
-    p.M = (int)rows; p.N = c.intermediate; p.K = c.hidden;
-    p.a = xn; p.lda = c.hidden; p.w = L.w_fc1; p.ldw = c.hidden;
-    p.out = u; p.ldo = c.intermediate; p.bias = L.b_fc1; p.epi = EPI_F16_BIAS_QGELU;
-    if (gemm_f16(p, sms, stream)) return 1;
-    p = GemmProblem{};
-    p.M = (int)rows; p.N = c.hidden; p.K = c.intermediate;
-    p.a = u; p.lda = c.intermediate; p.w = L.w_fc2; p.ldw = c.intermediate;
-    p.out = x; p.ldo = c.hidden; p.bias = L.b_fc2; p.epi = EPI_F32_BIAS_RESID;
-    if (gemm_f16(p, sms, stream)) return 1;
-  }
+  if (!folded && encoder_layers(h->layers.data(), c.layers, c.hidden, c.heads, c.intermediate, c.ln_eps, x, xn, u, n_views,
+                                h->tokens, nullptr, 0, sms, stream))
+    return 1;
   if (token_mean(x, emb_out, n_views, h->tokens, c.hidden, stream)) return 1;
   if (hidden_out) {
     cudaError_t e = cudaMemcpyAsync(hidden_out, x, (size_t)rows * c.hidden * sizeof(float), cudaMemcpyDeviceToDevice, stream);
     if (e != cudaSuccess) { set_last_error("pg_vit_forward: hidden copy: %s", cudaGetErrorString(e)); return 1; }
   }
+  if (cls_out) {   // row 0 of every view: one strided copy out of the residual stream
+    const size_t row_bytes = (size_t)c.hidden * sizeof(float);
+    cudaError_t e = cudaMemcpy2DAsync(cls_out, row_bytes, x, (size_t)h->tokens * row_bytes, row_bytes, n_views,
+                                      cudaMemcpyDeviceToDevice, stream);
+    if (e != cudaSuccess) { set_last_error("pg_vit_forward_cls: CLS copy: %s", cudaGetErrorString(e)); return 1; }
+  }
   return 0;
+}
+
+int pg_vit_forward(pg_vit* h, const void* pixels, int32_t pixels_f16, int32_t n_views, void* workspace,
+                   size_t workspace_bytes, float* emb_out, float* hidden_out, void* stream) {
+  return vit_forward(h, pixels, pixels_f16, n_views, workspace, workspace_bytes, emb_out, hidden_out, nullptr, stream);
+}
+
+int pg_vit_forward_cls(pg_vit* h, const void* pixels, int32_t pixels_f16, int32_t n_views, void* workspace,
+                       size_t workspace_bytes, float* emb_out, float* hidden_out, float* cls_out, void* stream) {
+  if (!cls_out) { set_last_error("pg_vit_forward_cls: null cls_out"); return 1; }
+  return vit_forward(h, pixels, pixels_f16, n_views, workspace, workspace_bytes, emb_out, hidden_out, cls_out, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- head
@@ -506,6 +536,13 @@ int pg_layernorm_f16(const float* x, void* y, const float* gamma, const float* b
 int pg_attention_f16(const void* qkv, void* out, int32_t n_views, int32_t seq, int32_t heads, void* stream) {
   if (!qkv || !out) { set_last_error("pg_attention_f16: null argument"); return 1; }
   return attention_f16(qkv, out, n_views, seq, heads, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pg_attention_f16_masked(const void* qkv, void* out, const int64_t* mask, int32_t causal, int32_t n_views, int32_t seq,
+                            int32_t heads, void* stream) {
+  if (!qkv || !out) { set_last_error("pg_attention_f16_masked: null argument"); return 1; }
+  return attention_f16_masked(qkv, out, reinterpret_cast<const long long*>(mask), causal, n_views, seq, heads,
+                              reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pg_attention_f16_variant(const void* qkv, void* out, float* lse2, int32_t n_views, int32_t seq, int32_t heads,

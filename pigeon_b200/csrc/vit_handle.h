@@ -21,6 +21,12 @@ namespace pg {
 
 int sm_count();   // cached cudaDevAttrMultiProcessorCount of the current device, -1 (and last_error) on failure
 
+// The pre-LN encoder-layer stack with LayerNorm kernels (capi.cu), shared by the vision tower (mask NULL, causal 0) and the
+// text tower (attention_mask, causal 1).  x f32 [n_seq * seq, hidden]; xn fp16 [rows, hidden]; u fp16 [rows, max(3 hidden,
+// intermediate)].
+int encoder_layers(const pg_vit_layer* layers, int n_layers, int hidden, int heads, int intermediate, float eps, float* x,
+                   void* xn, void* u, int n_seq, int seq, const int64_t* mask, int causal, int sms, cudaStream_t stream);
+
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 struct Carver {

@@ -1,10 +1,11 @@
 // Memory-bound pieces of the CLIP vision tower around the wgmma GEMM / attention kernels:
 // patch extraction (im2col), class-token + position embedding + pre_layrnorm, per-block LayerNorm,
-// and the token mean-pool that the reference applies to last_hidden_state
-// (models/clip_embedder.py:64-65, models/super_guessr.py:396-398).
+// the token mean-pool that the reference applies to last_hidden_state
+// (models/clip_embedder.py:64-65, models/super_guessr.py:396-398), and the text tower's token + position embedding.
 #include "vit_misc.h"
 
 #include <cuda_fp16.h>
+#include <limits.h>
 #include <stdint.h>
 
 #include "prof.h"
@@ -165,6 +166,105 @@ __global__ void embed_preln_kernel(float* __restrict__ x, const float* __restric
   }
 }
 
+// Text embeddings (HF CLIPTextEmbeddings, modeling_clip.py 4.23.1): x fp32 [n * S, hidden] row (b, t) =
+// token_embedding[ids[b, t]] + position_embedding[t].  No LayerNorm follows (the text tower has no pre-LN).  An id outside
+// [0, vocab) is never used as an index: its row becomes NaN, which is loud where HF raises an index error.
+__global__ void text_embed_kernel(const long long* __restrict__ ids, const float* __restrict__ tok,
+                                  const float* __restrict__ pos, float* __restrict__ x, long rows, int S, int hidden,
+                                  int vocab) {
+  const int lane = threadIdx.x & 31;
+  const int h4 = hidden >> 2;
+  const long warps = ((long)gridDim.x * blockDim.x) >> 5;
+  for (long row = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
+    const long long id = ids[row];
+    const bool ok = id >= 0 && id < vocab;
+    const float4* tr = reinterpret_cast<const float4*>(tok + (ok ? id : 0) * (long)hidden);
+    const float4* pr = reinterpret_cast<const float4*>(pos + (long)(row % S) * hidden);
+    float4* xr = reinterpret_cast<float4*>(x + row * hidden);
+    for (int i = lane; i < h4; i += 32) {
+      const float4 a = __ldg(tr + i), p = __ldg(pr + i);
+      xr[i] = ok ? make_float4(a.x + p.x, a.y + p.y, a.z + p.z, a.w + p.w) : make_float4(NAN, NAN, NAN, NAN);
+    }
+  }
+}
+
+// Final LayerNorm of the text tower in fp32 (HF CLIPTextTransformer.final_layer_norm), row by row:
+//   ids == nullptr: y[r] = LN(x[r])                                 (last_hidden_state, rows = n * S)
+//   ids != nullptr: y[r] = LN(x[r * S + argmax_t ids[r, t]])         (pooled output, rows = n; first index of the largest
+//                   id, transformers 4.23.1 `input_ids.argmax(dim=-1)`; the LayerNorm is per row, so pooling before or
+//                   after it gives the same row)
+template <int NV4>
+__global__ void rows_layernorm_f32_kernel(const float* __restrict__ x, float* __restrict__ y, const float* __restrict__ g,
+                                          const float* __restrict__ b, long rows, float eps,
+                                          const long long* __restrict__ ids, int S) {
+  constexpr int hidden = NV4 * 128;
+  const int lane = threadIdx.x & 31;
+  const long warps = ((long)gridDim.x * blockDim.x) >> 5;
+  for (long row = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
+    long src = row;
+    if (ids != nullptr) {
+      const long long* ir = ids + row * S;
+      long long bv = LLONG_MIN;
+      int bt = S;
+      for (int t = lane; t < S; t += 32) {
+        const long long v = ir[t];
+        if (v > bv) { bv = v; bt = t; }   // ascending t per lane: the first maximum of the lane
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const long long ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int ot = __shfl_xor_sync(0xffffffffu, bt, o);
+        if (ov > bv || (ov == bv && ot < bt)) { bv = ov; bt = ot; }
+      }
+      src = row * S + bt;
+    }
+    float4 v[NV4];
+    const float4* xr = reinterpret_cast<const float4*>(x + src * hidden);
+#pragma unroll
+    for (int i = 0; i < NV4; ++i) v[i] = xr[lane + 32 * i];
+    ln_row<NV4>(v, g, b, hidden, eps, lane);
+    float4* yr = reinterpret_cast<float4*>(y + row * hidden);
+#pragma unroll
+    for (int i = 0; i < NV4; ++i) yr[lane + 32 * i] = v[i];
+  }
+}
+
+// Operand of the error-compensated projection GEMM (the geocell head's scheme, head.cu): optional fp32 LayerNorm
+// (g == nullptr: none), then x = hi + lo in fp16 and a3 [rows, 3 * hidden] = [hi | lo | hi], to be multiplied by the
+// [Whi | Whi | Wlo] packing of pg_head_pack_weight.
+template <int NV4>
+__global__ void ln_split3_kernel(const float* __restrict__ x, __half* __restrict__ a3, const float* __restrict__ g,
+                                 const float* __restrict__ b, long rows, float eps) {
+  constexpr int hidden = NV4 * 128;
+  const int lane = threadIdx.x & 31;
+  const long warps = ((long)gridDim.x * blockDim.x) >> 5;
+  for (long row = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
+    float4 v[NV4];
+    const float4* xr = reinterpret_cast<const float4*>(x + row * hidden);
+#pragma unroll
+    for (int i = 0; i < NV4; ++i) v[i] = xr[lane + 32 * i];
+    if (g != nullptr) ln_row<NV4>(v, g, b, hidden, eps, lane);
+    uint2* hr = reinterpret_cast<uint2*>(a3 + row * 3 * hidden);
+    uint2* lr = reinterpret_cast<uint2*>(a3 + row * 3 * hidden + hidden);
+    uint2* h2 = reinterpret_cast<uint2*>(a3 + row * 3 * hidden + 2 * hidden);
+#pragma unroll
+    for (int i = 0; i < NV4; ++i) {
+      const __half2 h01 = __floats2half2_rn(v[i].x, v[i].y), h23 = __floats2half2_rn(v[i].z, v[i].w);
+      const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
+      const __half2 l01 = __floats2half2_rn(v[i].x - f01.x, v[i].y - f01.y);
+      const __half2 l23 = __floats2half2_rn(v[i].z - f23.x, v[i].w - f23.y);
+      uint2 ph, pl;
+      ph.x = *reinterpret_cast<const uint32_t*>(&h01);
+      ph.y = *reinterpret_cast<const uint32_t*>(&h23);
+      pl.x = *reinterpret_cast<const uint32_t*>(&l01);
+      pl.y = *reinterpret_cast<const uint32_t*>(&l23);
+      hr[lane + 32 * i] = ph;
+      lr[lane + 32 * i] = pl;
+      h2[lane + 32 * i] = ph;
+    }
+  }
+}
+
 // mean over tokens: x fp32 [n_views, tokens, hidden] -> out fp32 [n_views, hidden]
 // block = (hidden/4 threads, 1); each thread owns 4 adjacent columns; grid = (n_views, splits) with
 // partial sums combined through shared memory when blockDim.y > 1.
@@ -261,6 +361,35 @@ int embed_preln(float* x, const float* cls, const float* pos, const float* gamma
                                                                                reinterpret_cast<float2*>(stats),
                                                                                hidden / 128)));
   return check_launch("embed_preln");
+}
+
+int rows_layernorm_f32(const float* x, float* y, const float* gamma, const float* beta, long rows, int hidden, float eps,
+                       const long long* ids, int S, int num_sms, cudaStream_t stream) {
+  if (hidden % 128) { set_last_error("rows_layernorm_f32: hidden %d not a multiple of 128", hidden); return 1; }
+  const int grid = grid_for(rows, 8, num_sms);
+  ProfScope prof(ids ? "text_pool_ln" : "layernorm_f32", stream);
+  PG_DISPATCH_NV4(hidden, (rows_layernorm_f32_kernel<NV4><<<grid, 256, 0, stream>>>(x, y, gamma, beta, rows, eps, ids, S)));
+  return check_launch("rows_layernorm_f32");
+}
+
+int ln_split3(const float* x, void* a3, const float* gamma, const float* beta, long rows, int hidden, float eps, int num_sms,
+              cudaStream_t stream) {
+  if (hidden % 128) { set_last_error("ln_split3: hidden %d not a multiple of 128", hidden); return 1; }
+  if ((gamma == nullptr) != (beta == nullptr)) { set_last_error("ln_split3: LayerNorm gamma and beta go together"); return 1; }
+  const int grid = grid_for(rows, 8, num_sms);
+  ProfScope prof("clip_project_split", stream);
+  PG_DISPATCH_NV4(hidden, (ln_split3_kernel<NV4><<<grid, 256, 0, stream>>>(x, reinterpret_cast<__half*>(a3), gamma, beta,
+                                                                             rows, eps)));
+  return check_launch("ln_split3");
+}
+
+int text_embed(const long long* ids, const float* tok, const float* pos, float* x, long rows, int S, int hidden, int vocab,
+               int num_sms, cudaStream_t stream) {
+  if (hidden % 4) { set_last_error("text_embed: hidden %d not a multiple of 4", hidden); return 1; }
+  const int grid = grid_for(rows, 8, num_sms);
+  ProfScope prof("text_embed", stream);
+  text_embed_kernel<<<grid, 256, 0, stream>>>(ids, tok, pos, x, rows, S, hidden, vocab);
+  return check_launch("text_embed");
 }
 
 int token_mean(const float* x, float* out, int n_views, int tokens, int hidden, cudaStream_t stream) {

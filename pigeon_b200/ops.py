@@ -65,6 +65,74 @@ def attention_f16(qkv: torch.Tensor, n_views: int, seq: int, heads: int, variant
     return (out, lse2) if return_lse2 else out
 
 
+def attention_f16_masked(qkv: torch.Tensor, n_views: int, seq: int, heads: int, mask: torch.Tensor | None = None,
+                         causal: bool = False) -> torch.Tensor:
+    """The text tower's attention: qkv fp16 [n_views*seq, 3*heads*64] -> fp16 [n_views*seq, heads*64] with key j admissible
+    for query i only if (not causal or j <= i) and mask[view, j] != 0; mask i64 [n_views, seq] or None (mask[:, 0] must be
+    1).  No mask and causal=False is `attention_f16`."""
+    if mask is not None:
+        mask = mask.to(torch.int64).contiguous()
+    _need_cuda(qkv, mask)
+    assert qkv.dtype == torch.float16 and qkv.shape == (n_views * seq, 3 * heads * 64)
+    assert mask is None or mask.shape == (n_views, seq)
+    out = torch.empty((n_views * seq, heads * 64), dtype=torch.float16, device=qkv.device)
+    check(load().pg_attention_f16_masked(ptr(qkv), ptr(out), ptr(mask), int(bool(causal)), n_views, seq, heads,
+                                         current_stream_ptr()), "pg_attention_f16_masked")
+    return out
+
+
+def clip_project(x: torch.Tensor, w3: torch.Tensor, ln_weight: torch.Tensor | None = None,
+                 ln_bias: torch.Tensor | None = None, eps: float = 1e-5) -> torch.Tensor:
+    """x f32 [n, D] -> f32 [n, P] = LN(x) W^T (LN only when ln_weight / ln_bias are given), W packed by `head_pack_weight`
+    into w3 fp16 [P, 3*D]: the error-compensated split GEMM of the geocell head (visual_projection / text_projection)."""
+    _need_cuda(x, w3, ln_weight, ln_bias)
+    if (ln_weight is None) != (ln_bias is None):
+        raise ValueError("ln_weight and ln_bias go together")
+    assert x.dtype == torch.float32 and x.dim() == 2 and w3.dtype == torch.float16
+    n, D = x.shape
+    P = w3.shape[0]
+    if w3.shape[1] != 3 * D:
+        raise PigeonB200Error(f"packed weight {tuple(w3.shape)} does not match input dim {D}")
+    lib = load()
+    out = torch.empty((n, P), dtype=torch.float32, device=x.device)
+    if n == 0:
+        return out
+    ws = torch.empty(lib.pg_clip_project_workspace_bytes(n, D), dtype=torch.uint8, device=x.device)
+    check(lib.pg_clip_project(ptr(x), n, D, ptr(ln_weight), ptr(ln_bias), float(eps), ptr(w3), P, ptr(ws), ws.numel(),
+                              ptr(out), current_stream_ptr()), "pg_clip_project")
+    return out
+
+
+def clip_logits(image_embeds: torch.Tensor, text_embeds: torch.Tensor, logit_scale: float, per_text: bool = True,
+                probs: bool = False, pred: bool = False, loss: bool = False) -> dict:
+    """CLIPModel's logits from UNnormalised embeds (normalised inside): image_embeds f32 [Ni, P], text_embeds f32 [Nt, P]
+    -> dict(logits_per_image [Ni, Nt] and, on request, logits_per_text [Nt, Ni], probs [Ni, Nt] (softmax over captions),
+    pred i64 [Ni] (first argmax), loss f32 [] (symmetric cross-entropy against arange; needs Ni == Nt))."""
+    img = image_embeds.to(torch.float32).contiguous()
+    txt = text_embeds.to(torch.float32).contiguous()
+    _need_cuda(img, txt)
+    Ni, P = img.shape
+    Nt = txt.shape[0]
+    if txt.shape[1] != P:
+        raise ValueError(f"image embeds have dim {P}, text embeds {txt.shape[1]}")
+    if loss and Ni != Nt:
+        raise ValueError(f"the contrastive loss needs as many images as captions (got {Ni} images, {Nt} captions)")
+    dev = img.device
+    out = dict(logits_per_image=torch.empty((Ni, Nt), dtype=torch.float32, device=dev))
+    if per_text:
+        out["logits_per_text"] = torch.empty((Nt, Ni), dtype=torch.float32, device=dev)
+    if probs:
+        out["probs"] = torch.empty((Ni, Nt), dtype=torch.float32, device=dev)
+    if pred:
+        out["pred"] = torch.empty((Ni,), dtype=torch.int64, device=dev)
+    if loss:
+        out["loss"] = torch.empty((), dtype=torch.float32, device=dev)
+    check(load().pg_clip_logits(ptr(img), Ni, ptr(txt), Nt, P, float(logit_scale), ptr(out["logits_per_image"]),
+                                ptr(out.get("logits_per_text")), ptr(out.get("probs")), ptr(out.get("pred")),
+                                ptr(out.get("loss")), current_stream_ptr()), "pg_clip_logits")
+    return out
+
+
 def refiner_scan(bank: "DeviceBank", emb: torch.Tensor, cand_idx: torch.Tensor, topk: int):
     """Scan stage only (cell-sharded banks): per (query, candidate) partials (best_logit [B, topk], best_lnglat
     [B, topk, 2], best_proto [B, topk]); pairs whose geocell this bank does not hold come back as -100000 / (0, 0) / -1."""

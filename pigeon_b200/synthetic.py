@@ -42,6 +42,42 @@ def random_vit_state_dict(dims: VitDims, seed: int = 0, std: float = 0.02) -> Di
     return sd
 
 
+def random_clip_state_dict(text_dims, vision_dims: VitDims, seed: int = 0, std: float = 0.02,
+                           projection_dim: Optional[int] = None) -> Dict[str, torch.Tensor]:
+    """HF-named CLIPModel state dict: `random_vit_state_dict(vision_dims, seed)` for `vision_model.*`, N(0, std) text tower
+    (`text_model.*`, unit-ish LayerNorms, small biases), bias-free projections to `projection_dim` (default: the text
+    width, as in CLIP-L/14) and logit_scale = log(1 / 0.07)."""
+    sd = random_vit_state_dict(vision_dims, seed=seed, std=std)
+    g = torch.Generator().manual_seed(seed + 7919)
+    P = text_dims.hidden if projection_dim is None else projection_dim
+    H = text_dims.hidden
+
+    def n(*shape, s=std):
+        return torch.randn(*shape, generator=g) * s
+
+    sd["text_model.embeddings.token_embedding.weight"] = n(text_dims.vocab, H)
+    sd["text_model.embeddings.position_embedding.weight"] = n(text_dims.max_positions, H)
+    for i in range(text_dims.layers):
+        p = f"text_model.encoder.layers.{i}."
+        for nm in ("q_proj", "k_proj", "v_proj", "out_proj"):
+            sd[p + f"self_attn.{nm}.weight"] = n(H, H)
+            sd[p + f"self_attn.{nm}.bias"] = n(H)
+        sd[p + "layer_norm1.weight"] = 1 + n(H)
+        sd[p + "layer_norm1.bias"] = n(H)
+        sd[p + "layer_norm2.weight"] = 1 + n(H)
+        sd[p + "layer_norm2.bias"] = n(H)
+        sd[p + "mlp.fc1.weight"] = n(text_dims.intermediate, H)
+        sd[p + "mlp.fc1.bias"] = n(text_dims.intermediate)
+        sd[p + "mlp.fc2.weight"] = n(H, text_dims.intermediate)
+        sd[p + "mlp.fc2.bias"] = n(H)
+    sd["text_model.final_layer_norm.weight"] = 1 + n(H)
+    sd["text_model.final_layer_norm.bias"] = n(H)
+    sd["visual_projection.weight"] = n(P, vision_dims.hidden)
+    sd["text_projection.weight"] = n(P, H)
+    sd["logit_scale"] = torch.tensor(float(np.log(1 / 0.07)), dtype=torch.float32)
+    return sd
+
+
 def synthetic_geocells(num_cells: int, seed: int = 0) -> np.ndarray:
     """(C, 2) float64 (lng, lat): lng ~ U(-180, 180), lat ~ U(-90, 90)   (SURVEY.md §8d cfg1)."""
     rng = np.random.default_rng(seed)

@@ -191,6 +191,31 @@ class VitEngine:
         return (emb, hidden) if return_hidden else emb
 
     @torch.no_grad()
+    def forward_cls(self, pixel_values: torch.Tensor):
+        """pixel_values [N, 3, H, W] (fp32 or fp16; host tensors are copied over first) -> (token-mean embedding [N, hidden],
+        CLS rows of last_hidden_state [N, hidden]) fp32, through pg_vit_forward_cls: the CLS rows that CLIPModel's image
+        features start from, without the [N, tokens, hidden] last_hidden_state."""
+        d = self.dims
+        if pixel_values.dim() != 4 or tuple(pixel_values.shape[1:]) != (3, d.image_size, d.image_size):
+            raise ValueError(f"Input image size ({tuple(pixel_values.shape[1:])}) doesn't match model "
+                             f"(3, {d.image_size}, {d.image_size}).")
+        if pixel_values.dtype not in (torch.float32, torch.float16):
+            pixel_values = pixel_values.float()
+        pixel_values = pixel_values.to(self.device).contiguous()
+        n = pixel_values.shape[0]
+        emb = torch.empty((n, d.hidden), dtype=torch.float32, device=self.device)
+        cls = torch.empty((n, d.hidden), dtype=torch.float32, device=self.device)
+        step = max(1, min(self.max_views_per_pass, n))
+        ws = self._workspace(step)
+        stream = current_stream_ptr()
+        for s in range(0, n, step):
+            e = min(n, s + step)
+            check(self._lib.pg_vit_forward_cls(self._handle, ptr(pixel_values[s:e]), int(pixel_values.dtype == torch.float16),
+                                               e - s, ptr(ws), ws.numel(), ptr(emb[s:e]), None, ptr(cls[s:e]), stream),
+                  "pg_vit_forward_cls")
+        return emb, cls
+
+    @torch.no_grad()
     def _forward_from_host(self, pixel_values: torch.Tensor, return_hidden: bool, host_chunk: int = 256):
         """Host (ideally pinned) pixels: the H2D copy of chunk i+1 runs on a side stream while chunk i computes,
         through two device staging buffers (the reference copies the whole batch up front, super_guessr.py:193-217)."""
