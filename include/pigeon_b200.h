@@ -274,6 +274,57 @@ size_t pg_vit_backward_workspace_bytes(const pg_vit* h, int32_t n_views);
 int pg_vit_backward(pg_vit* h, const pg_vit_saved* saved, const float* d_emb, int32_t n_views, const pg_vit_grads* grads,
                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* As pg_vit_backward, but d_cls f32 [n_views, hidden] is the gradient of the CLS rows last_hidden_state[:, 0] (HF
+ * CLIPVisionTransformer's pooled output, transformers 4.23.1 modeling_clip.py `pooled_output = last_hidden_state[:, 0, :]`,
+ * which CLIPModel.get_image_features feeds to post_layernorm and visual_projection): the backward starts from d_cls at
+ * token 0 of each view and zero elsewhere.  Same saved activations (x_out holds the CLS rows) and workspace. */
+int pg_vit_backward_cls(pg_vit* h, const pg_vit_saved* saved, const float* d_cls, int32_t n_views, const pg_vit_grads* grads,
+                        void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
+ * CLIPModel contrastive training step: what autograd runs through HF CLIPModel (transformers 4.23.1 modeling_clip.py) for
+ * `loss.backward()` under the HF Trainer of reference training/train_modes.py:30-64 (`return_loss=True`, nothing frozen).
+ * The text tower reuses the vision tower's saved-activation layout and encoder-layer backward (causal + attention_mask
+ * attention); the projections' backward is pg_head_backward with db = NULL, post_layernorm's pg_layernorm_f32 /
+ * pg_layernorm_backward, the vision side pg_vit_forward_train + pg_vit_backward_cls.
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct pg_text_saved {
+  float* x_final;                         /* f32 [n*S, hidden] residual stream entering final_layer_norm */
+  const pg_vit_saved_layer* layers_host;  /* [layers], rows = n*S (x0 of layer 0 = the embeddings; lse2 [n*heads, S]) */
+} pg_text_saved;
+
+typedef struct pg_text_grads {
+  float* d_token_emb;    /* f32 [vocab, hidden]          (+=) embeddings.token_embedding.weight */
+  float* d_pos_emb;      /* f32 [max_positions, hidden]  (+=) embeddings.position_embedding.weight (rows >= S untouched) */
+  float* d_final_ln_g;   /* f32 [hidden] (+=) */
+  float* d_final_ln_b;   /* f32 [hidden] (+=) */
+  const pg_vit_layer_bwd* layers_host;  /* [layers]: every layer's gradients are required */
+} pg_text_grads;
+
+/* pg_text_forward with the activations the backward needs kept in `saved` (HF CLIPTextTransformer.forward):
+ * pooled_out f32 [n, hidden] = final_layer_norm(x)[b, argmax_t input_ids[b, t]]. */
+int pg_text_forward_train(pg_text* h, const int64_t* input_ids, const int64_t* attention_mask, int32_t n, int32_t S,
+                          const pg_text_saved* saved, float* pooled_out, void* stream);
+size_t pg_text_backward_workspace_bytes(const pg_text* h, int32_t n, int32_t S);
+/* d_pooled f32 [n, hidden] (gradient of pooled_out) with the input_ids / attention_mask of the forward -> every text-tower
+ * gradient (+=): final_layer_norm on the pooled rows, the encoder layers, d position_embedding[:S] = sums over captions,
+ * d token_embedding = per-id sums over the n*S rows in a fixed order (deterministic; ids outside [0, vocab) skipped). */
+int pg_text_backward(pg_text* h, const pg_text_saved* saved, const int64_t* input_ids, const int64_t* attention_mask,
+                     const float* d_pooled, int32_t n, int32_t S, const pg_text_grads* grads, void* workspace,
+                     size_t workspace_bytes, void* stream);
+
+/* clip_loss of HF CLIPModel.forward (modeling_clip.py 4.23.1 `clip_loss(logits_per_text)`) and its gradient, for n images
+ * and n captions: img, txt f32 [n, P] (projected, not normalised), logit_scale: DEVICE f32 scalar (the parameter; s = exp)
+ *   -> loss f32 [1];  d_img, d_txt f32 [n, P] and d_logit_scale f32 [1] (overwritten, times grad_scale), with
+ *      L = s T^ I^T, dL = (softmax_rows(L) - 1 + softmax_cols(L) - 1) / 2n, dT^ = s dL I^, dI^ = s dL^T T^,
+ *      d logit_scale = sum dL o L, dT = (dT^ - T^ (T^ . dT^)) / |T| (and the same for I);
+ *   -> optional (NULL = not written) logits_per_image / logits_per_text f32 [n, n].
+ * Products and normalisation in fp32, sums and the softmax in fp64; deterministic. */
+size_t pg_clip_loss_grad_workspace_bytes(int32_t n, int32_t P);
+int pg_clip_loss_grad(const float* img, const float* txt, int32_t n, int32_t P, const float* logit_scale, double grad_scale,
+                      void* workspace, size_t workspace_bytes, float* loss, float* d_img, float* d_txt, float* d_logit_scale,
+                      float* logits_per_image, float* logits_per_text, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * ProtoRefiner (reference models/proto_refiner.py:121-255, 332-357; preprocessing/geo_utils.py:40-55)
  * ------------------------------------------------------------------------------------------------- */
@@ -403,6 +454,19 @@ int pg_attention_f16_lse(const void* qkv, void* out, float* lse2, int32_t n_view
 size_t pg_attention_backward_workspace_bytes(int32_t n_views, int32_t seq, int32_t heads);
 int pg_attention_backward(const void* qkv, const void* out, const float* d_out, const float* lse2, void* dqkv_bf16,
                           int32_t n_views, int32_t seq, int32_t heads, void* workspace, size_t workspace_bytes, void* stream);
+/* pg_attention_f16_masked also writing lse2 f32 [n_views*heads, seq] over the admissible keys (the text tower's training
+ * forward). */
+int pg_attention_f16_masked_lse(const void* qkv, void* out, float* lse2, const int64_t* mask, int32_t causal, int32_t n_views,
+                                int32_t seq, int32_t heads, void* stream);
+/* pg_attention_backward of the masked attention (same admissibility as pg_attention_f16_masked; lse2 from
+ * pg_attention_f16_masked_lse).  mask NULL and causal 0 is pg_attention_backward, bit for bit. */
+int pg_attention_backward_masked(const void* qkv, const void* out, const float* d_out, const float* lse2, const int64_t* mask,
+                                 int32_t causal, void* dqkv_bf16, int32_t n_views, int32_t seq, int32_t heads, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+/* fp32 LayerNorm: x f32 [rows, hidden] -> y f32 [rows, hidden] (HF nn.LayerNorm in fp32; CLIPModel's post_layernorm input of
+ * the visual_projection weight gradient). */
+int pg_layernorm_f32(const float* x, float* y, const float* gamma, const float* beta, int64_t rows, int32_t hidden, float eps,
+                     void* stream);
 /* LayerNorm backward: dx (+)= dLN(x)/dx . dy;  dgamma / dbeta (both or neither NULL) += their gradients;
  * dx_bf16 (nullable): bf16 copy of the final dx, the operand of the next data-gradient GEMM. */
 int pg_layernorm_backward(const float* dy, const float* x, const float* gamma, float* dx, int32_t accumulate, float* dgamma,

@@ -36,6 +36,7 @@ SOURCES = [
     "capi.cu",
     "clip.cu",
     "clip_capi.cu",
+    "clip_train.cu",
 ]
 
 NVCC_FLAGS = [

@@ -68,6 +68,15 @@ class TextWeights(C.Structure):
                 ("final_ln_g", c_void_p), ("final_ln_b", c_void_p)]
 
 
+class TextSaved(C.Structure):
+    _fields_ = [("x_final", c_void_p), ("layers_host", C.POINTER(VitSavedLayer))]
+
+
+class TextGrads(C.Structure):
+    _fields_ = [("d_token_emb", c_void_p), ("d_pos_emb", c_void_p), ("d_final_ln_g", c_void_p), ("d_final_ln_b", c_void_p),
+                ("layers_host", C.POINTER(VitLayerBwd))]
+
+
 class RefinerBank(C.Structure):
     _fields_ = [("num_cells", c_int32), ("dim", c_int32), ("cell_off", c_void_p), ("proto_emb", c_void_p),
                 ("proto_lnglat", c_void_p), ("proto_count", c_void_p), ("member_off", c_void_p),
@@ -99,6 +108,21 @@ SIGNATURES = {
     "pg_vit_backward_workspace_bytes": (c_size_t, [c_void_p, c_int32]),
     "pg_vit_backward": (c_int32, [c_void_p, C.POINTER(VitSaved), c_void_p, c_int32, C.POINTER(VitGrads), c_void_p, c_size_t,
                                   c_void_p]),
+    "pg_vit_backward_cls": (c_int32, [c_void_p, C.POINTER(VitSaved), c_void_p, c_int32, C.POINTER(VitGrads), c_void_p,
+                                      c_size_t, c_void_p]),
+    "pg_text_forward_train": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, C.POINTER(TextSaved), c_void_p,
+                                        c_void_p]),
+    "pg_text_backward_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
+    "pg_text_backward": (c_int32, [c_void_p, C.POINTER(TextSaved), c_void_p, c_void_p, c_void_p, c_int32, c_int32,
+                                   C.POINTER(TextGrads), c_void_p, c_size_t, c_void_p]),
+    "pg_clip_loss_grad_workspace_bytes": (c_size_t, [c_int32, c_int32]),
+    "pg_clip_loss_grad": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_double, c_void_p, c_size_t, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pg_attention_f16_masked_lse": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
+                                              c_void_p]),
+    "pg_attention_backward_masked": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_int32,
+                                               c_int32, c_int32, c_void_p, c_size_t, c_void_p]),
+    "pg_layernorm_f32": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_float, c_void_p]),
     "pg_gemm_ex": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32,
                              c_int32, c_int32, c_int32, c_void_p]),
     "pg_gemm_tn": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,

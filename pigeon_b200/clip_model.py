@@ -4,7 +4,10 @@ training/train_modes.py:30-64 pretrains into StreetCLIP and that `PretrainDatase
 `model(**clip_processor(text=captions, images=images), return_loss=True).logits_per_image.softmax(1).argmax(1)`.
 
 Parameter names are HF's (`text_model.*`, `vision_model.*`, `visual_projection.weight`, `text_projection.weight`,
-`logit_scale`), so CLIPModel checkpoints load by name.  Forward only: the pretraining step is not implemented.
+`logit_scale`), so CLIPModel checkpoints load by name.
+
+`forward_train` + `backward` is one contrastive training step (the gradient of `clip_loss` for every parameter, for
+`training.AdamW`); the HF Trainer around it (schedule, clipping, checkpoints) is not implemented.
 
     image features = visual_projection(post_layernorm(last_hidden_state[:, 0]))      (CLS row; pg_vit_forward_cls)
     text features  = text_projection(pooled)                                          (pg_text_forward)
@@ -24,9 +27,11 @@ from torch.nn.parameter import Parameter
 
 from . import _versions, ops
 from ._lib import PigeonB200Error
+from ._lib import check, current_stream_ptr, load, ptr
 from .clip_text import CLIPTextTower, TextDims, _Holder, check_sequence_length
 from .super_guessr import CLIPVisionTower
 from .vit_engine import VitDims
+from .vit_train import put_grad
 
 LOGIT_SCALE_INIT = math.log(1 / 0.07)   # CLIPConfig.logit_scale_init_value (2.6592)
 
@@ -58,6 +63,8 @@ class CLIPModel(nn.Module):
         self.text_projection.weight = Parameter(torch.zeros(projection_dim, text_dims.hidden))
         self.logit_scale = Parameter(torch.tensor(LOGIT_SCALE_INIT))
         self._packed = {}
+        self.max_train_views = 64    # activation arena of the vision tower's training step (about 0.52 GB per ViT-L/14-336 view)
+        self._pend = None
 
     @property
     def text_tower(self) -> CLIPTextTower:
@@ -141,3 +148,111 @@ class CLIPModel(nn.Module):
                           logits_per_text=out["logits_per_text"],
                           text_embeds=text_features / text_features.norm(p=2, dim=-1, keepdim=True),
                           image_embeds=image_features / image_features.norm(p=2, dim=-1, keepdim=True))
+
+    # ------------------------------------------------------------------------------------------ training step
+    def _trainers(self):
+        from .clip_train import TextTrainer
+        from .vit_train import TowerTrainer
+        tr = getattr(self, "_vision_trainer", None)
+        if tr is None or tr.tower is not self.vision_tower or tr.max_views != self.max_train_views:
+            tr = self._vision_trainer = TowerTrainer(self.vision_tower, max_views=self.max_train_views)
+        tt = getattr(self, "_text_trainer", None)
+        if tt is None or tt.tower is not self.text_tower:
+            tt = self._text_trainer = TextTrainer(self.text_tower)
+        return tr, tt
+
+    def forward_train(self, input_ids: Tensor, pixel_values: Tensor, attention_mask: Optional[Tensor] = None) -> CLIPOutput:
+        """One contrastive step of HF CLIPModel (`model(input_ids, pixel_values, attention_mask, return_loss=True)` then
+        `loss.backward()`, as the HF Trainer of reference training/train_modes.py:30-64 runs it): the forward, the loss
+        `clip_loss(logits_per_text)` over n images and n captions, and every parameter gradient, kept pending in fp32
+        buffers until `backward()` publishes them.  The vision tower follows `TowerTrainer`'s freeze rules; every text-tower
+        parameter must be trainable.  n <= max_train_views (one activation arena; no chunking)."""
+        self._check_cuda()
+        if input_ids is None or pixel_values is None:
+            raise ValueError("CLIPModel.forward_train needs both input_ids and pixel_values")
+        if input_ids.dim() != 2:
+            raise ValueError(f"input_ids must be [batch, sequence], got {tuple(input_ids.shape)}")
+        n, S = input_ids.shape
+        check_sequence_length(S, self.text_dims.max_positions)
+        if pixel_values.shape[0] != n:
+            raise ValueError(f"the contrastive loss needs as many images as captions (got {pixel_values.shape[0]} images, "
+                             f"{n} captions)")
+        if attention_mask is not None and tuple(attention_mask.shape) != (n, S):
+            raise ValueError(f"attention_mask {tuple(attention_mask.shape)} does not match input_ids {(n, S)}")
+        tr, tt = self._trainers()
+        if n > tr.max_views:
+            raise PigeonB200Error(f"{n} image-caption pairs exceed max_views={tr.max_views} of the training arena (a "
+                                  f"contrastive batch is not split into chunks)")
+        if n == 0:
+            raise ValueError("forward_train needs at least one image-caption pair")
+        tt.check_trainable()
+        tr.layout()                                                      # raises if a block is only partly trainable
+        dev = self.logit_scale.device
+        vis_trains = tr.any_trainable()
+        post = self.vision_model.post_layernorm
+        eps = self.vision_dims.ln_eps
+        Wv, Wt = self.visual_projection.weight, self.text_projection.weight
+        lib = load()
+        stream = current_stream_ptr()
+        with torch.no_grad():
+            # forward: CLS rows -> post_layernorm -> visual_projection; pooled text row -> text_projection
+            px = pixel_values.to(dev)
+            if px.dtype not in (torch.float16, torch.float32):
+                px = px.float()
+            tr.forward(px)
+            cls = tr.cls_rows()
+            pv = ops.layernorm_f32(cls, post.weight.detach(), post.bias.detach(), eps)
+            img = ops.clip_project(pv, self._packed_projection("visual_projection"))
+            pooled = tt.forward(input_ids.to(dev), None if attention_mask is None else attention_mask.to(dev))
+            txt = ops.clip_project(pooled, self._packed_projection("text_projection"))
+            out = ops.clip_loss_grad(img, txt, self.logit_scale)
+
+            # backward: projections (pg_head_backward, no bias), post_layernorm, then both towers
+            pend = {}
+
+            def grad_buf(p):
+                if not p.requires_grad:
+                    return None
+                pend[p] = torch.zeros_like(p, dtype=torch.float32)
+                return pend[p]
+
+            d_pv = torch.empty_like(pv)
+            d_pooled = torch.empty_like(pooled)
+            check(lib.pg_head_backward(ptr(out["d_image_embeds"]), ptr(pv), ptr(Wv.detach()), n, Wv.shape[0], Wv.shape[1], 1,
+                                       ptr(grad_buf(Wv)), None, ptr(d_pv), stream), "pg_head_backward")
+            check(lib.pg_head_backward(ptr(out["d_text_embeds"]), ptr(pooled), ptr(Wt.detach()), n, Wt.shape[0], Wt.shape[1],
+                                       1, ptr(grad_buf(Wt)), None, ptr(d_pooled), stream), "pg_head_backward")
+            if self.logit_scale.requires_grad:
+                pend[self.logit_scale] = out["d_logit_scale"]
+            dg, db = grad_buf(post.weight), grad_buf(post.bias)
+            if (dg is None) != (db is None):
+                raise PigeonB200Error("post_layernorm weight and bias must be trainable or frozen together")
+            if vis_trains:
+                d_cls = torch.empty_like(cls)
+                check(lib.pg_layernorm_backward(ptr(d_pv), ptr(cls), ptr(post.weight.detach()), ptr(d_cls), 0, ptr(dg), ptr(db),
+                                                None, n, cls.shape[1], eps, stream), "pg_layernorm_backward")
+                tr.backward_cls(d_cls)
+            elif dg is not None:
+                scratch = torch.empty_like(cls)
+                check(lib.pg_layernorm_backward(ptr(d_pv), ptr(cls), ptr(post.weight.detach()), ptr(scratch), 0, ptr(dg),
+                                                ptr(db), None, n, cls.shape[1], eps, stream), "pg_layernorm_backward")
+            tt.backward(d_pooled)
+        self._pend = (pend, vis_trains)
+        return CLIPOutput(loss=out["loss"], logits_per_image=out["logits_per_image"], logits_per_text=out["logits_per_text"],
+                          text_embeds=txt / txt.norm(p=2, dim=-1, keepdim=True),
+                          image_embeds=img / img.norm(p=2, dim=-1, keepdim=True))
+
+    @torch.no_grad()
+    def backward(self, loss: Optional[Tensor] = None) -> None:
+        """Publish the gradients of the last `forward_train` into `.grad` under the HF names, adding to any gradient already
+        there (gradient accumulation), like `SuperGuessr.backward`.  `loss` is accepted for the `loss.backward()` shape of
+        the call and not used."""
+        if self._pend is None:
+            raise PigeonB200Error("backward() needs a preceding forward_train()")
+        pend, vis_trains = self._pend
+        self._pend = None
+        for p, g in pend.items():
+            put_grad(p, g.reshape(p.shape))
+        if vis_trains:
+            self._vision_trainer.finalize(1)
+        self._text_trainer.finalize()

@@ -15,6 +15,11 @@
 //
 // One warpgroup (128 threads) per CTA; thread 0 keeps the three 64 x 64 tiles of the NEXT block in flight through a 2-slot
 // TMA ring.  P / dS are formed on the accumulator fragments of S / dP, which are the A-operand fragments of the next MMA.
+//
+// kMasked = true is the text tower's variant: the admissibility predicate of the masked forward (key j admissible for query i
+// only if j <= i when causal, and mask[view, j] != 0) zeroes P and dS on the recomputed S / S^T fragments.  With causal
+// masking a dQ row tile stops at its diagonal KV block and a dK/dV row tile starts at its diagonal query block
+// (kRows == kBlk, so the diagonal block index is the tile index).
 #include <cuda_bf16.h>
 
 #include "attention.h"
@@ -43,6 +48,8 @@ struct BwdArgs {
   __nv_bfloat16* dqkv;  // [n_views * seq, 3 * hidden]
   float scale;          // 1 / sqrt(64)
   float scale_log2;     // scale * log2(e)
+  const long long* mask;   // kMasked: optional [n_views, seq], 0 = key excluded
+  int causal;              // kMasked: key j admissible for query i only if j <= i
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -55,7 +62,7 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int MODE>
+template <int MODE, bool kMasked>
 __global__ void __launch_bounds__(kThreads, 2)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_f16, const __grid_constant__ CUtensorMap tmap_bf16,
                      const __grid_constant__ CUtensorMap tmap_do, const BwdArgs args) {
@@ -73,12 +80,18 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_f16, const __grid_
   const int tile = blockIdx.x, head = blockIdx.y, view = blockIdx.z;
   const int S = args.seq;
   const int heads = args.hidden / kHeadDim;
-  const int nb = (S + kBlk - 1) / kBlk;
+  int j0 = 0, nb = (S + kBlk - 1) / kBlk;   // column blocks [j0, nb)
+  if constexpr (kMasked) {
+    if (args.causal) {
+      if (MODE == MODE_DQ) nb = tile + 1;
+      else j0 = tile;
+    }
+  }
   const int row0 = view * S;
   const int q_col = head * kHeadDim, k_col = args.hidden + q_col, v_col = 2 * args.hidden + q_col;
 
   auto load_block = [&](int j) {   // thread 0 only
-    const int slot = j & 1;
+    const int slot = (j - j0) & 1;
     uint8_t* st = smem_st + slot * kSlotBytes;
     const int c_row = j * kBlk;
     mbar_arrive_expect_tx(&full_bar[slot], kSlotBytes);
@@ -110,7 +123,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_f16, const __grid_
       tma_load_3d(smem_r16, &tmap_f16, r_full, k_col, r_row, view);
       tma_load_3d(smem_rbf, &tmap_bf16, r_full, v_col, r_row, view);
     }
-    load_block(0);
+    load_block(j0);
   }
   __syncthreads();
 
@@ -128,10 +141,18 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_f16, const __grid_
   float acc1[32], acc2[32];   // dQ | dV, dK
 #pragma unroll
   for (int i = 0; i < 32; ++i) acc1[i] = acc2[i] = 0.f;
+  // kMasked: admissibility of this thread's two rows as keys (MODE_DKV)
+  bool key_a = true, key_b = true;
+  if constexpr (kMasked) {
+    if (MODE == MODE_DKV && args.mask) {
+      key_a = va && __ldg(args.mask + (size_t)view * S + r_a) != 0;
+      key_b = vb && __ldg(args.mask + (size_t)view * S + r_b) != 0;
+    }
+  }
   mbar_wait(r_full, 0);
 
-  for (int j = 0; j < nb; ++j) {
-    const int slot = j & 1;
+  for (int j = j0; j < nb; ++j) {
+    const int slot = (j - j0) & 1;
     if (threadIdx.x == 0 && j + 1 < nb) load_block(j + 1);   // slot (j + 1) & 1 was released by the barrier ending j - 1
     if (MODE == MODE_DKV) {
       // per-column statistics of this query block (columns past the view are masked below)
@@ -139,7 +160,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_f16, const __grid_
       cbuf[threadIdx.x] = qi < S ? (threadIdx.x < 64 ? args.lse2[stat0 + qi] : args.delta[stat0 + qi]) : 0.f;
       __syncthreads();
     }
-    mbar_wait(&full_bar[slot], (j >> 1) & 1);
+    mbar_wait(&full_bar[slot], ((j - j0) >> 1) & 1);
     const uint32_t c16 = smem_u32(smem_st + slot * kSlotBytes), cb1 = c16 + kTileBytes, cb2 = cb1 + kTileBytes;
 
     float sv[32], dv[32];
@@ -160,7 +181,17 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_f16, const __grid_
 #pragma unroll
       for (int e = 0; e < 4; ++e) {   // e & 1: column of the pair; e >> 1: row a / row b
         const int col = j * kBlk + 8 * g + 2 * (lane & 3) + (e & 1);   // index inside the view of this column
-        const bool ok = ((e >> 1) ? vb : va) && col < S;
+        bool ok = ((e >> 1) ? vb : va) && col < S;
+        if constexpr (kMasked) {
+          const int row = (e >> 1) ? r_b : r_a;
+          if (MODE == MODE_DQ) {       // row = query, col = key
+            if (args.causal) ok = ok && col <= row;
+            if (args.mask) ok = ok && __ldg(args.mask + (size_t)view * S + col) != 0;
+          } else {                     // row = key, col = query
+            if (args.causal) ok = ok && row <= col;
+            ok = ok && ((e >> 1) ? key_b : key_a);
+          }
+        }
         float lse, dl;
         if (MODE == MODE_DQ) { lse = (e >> 1) ? lse_b : lse_a; dl = (e >> 1) ? dl_b : dl_a; }
         else { lse = cbuf[col - j * kBlk]; dl = cbuf[kBlk + col - j * kBlk]; }
@@ -209,14 +240,15 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmap_f16, const __grid_
   }
 }
 
-template <int MODE>
+template <int MODE, bool kMasked = false>
 int launch_bwd(const CUtensorMap& t16, const CUtensorMap& tbf, const CUtensorMap& tdo, const BwdArgs& a, int n_views,
                int heads, cudaStream_t stream) {
-  auto kern = attention_bwd_kernel<MODE>;
+  auto kern = attention_bwd_kernel<MODE, kMasked>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
   if (e != cudaSuccess) { set_last_error("attention_backward: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return 1; }
   dim3 grid((a.seq + kRows - 1) / kRows, heads, n_views);
-  ProfScope prof(MODE == MODE_DQ ? "attention_bwd_dq" : "attention_bwd_dkv", stream);
+  ProfScope prof(MODE == MODE_DQ ? (kMasked ? "attention_bwd_dq_masked" : "attention_bwd_dq")
+                                 : (kMasked ? "attention_bwd_dkv_masked" : "attention_bwd_dkv"), stream);
   kern<<<grid, kThreads, kSmemBytes, stream>>>(t16, tbf, tdo, a);
   e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error("attention_backward launch: %s", cudaGetErrorString(e)); return 1; }
@@ -225,8 +257,11 @@ int launch_bwd(const CUtensorMap& t16, const CUtensorMap& tbf, const CUtensorMap
 
 }  // namespace
 
-int attention_backward(const void* qkv_f16, const void* qkv_bf16, const void* d_out_bf16, const float* lse2,
-                       const float* delta, void* dqkv_bf16, int n_views, int seq, int heads, cudaStream_t stream) {
+namespace {
+
+template <bool kMasked>
+int run_backward(const void* qkv_f16, const void* qkv_bf16, const void* d_out_bf16, const float* lse2, const float* delta,
+                 void* dqkv_bf16, const long long* mask, int causal, int n_views, int seq, int heads, cudaStream_t stream) {
   if (n_views <= 0) return 0;
   if (n_views > 65535) { set_last_error("attention_backward: n_views %d > 65535 (grid.z)", n_views); return 1; }
   const int hidden = heads * kHeadDim;
@@ -239,8 +274,26 @@ int attention_backward(const void* qkv_f16, const void* qkv_bf16, const void* d_
   a.dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv_bf16);
   a.scale = 0.125f;
   a.scale_log2 = 0.125f * 1.4426950408889634f;
-  if (launch_bwd<MODE_DQ>(t16, tbf, tdo, a, n_views, heads, stream)) return 1;
-  return launch_bwd<MODE_DKV>(t16, tbf, tdo, a, n_views, heads, stream);
+  a.mask = mask;
+  a.causal = causal;
+  if (launch_bwd<MODE_DQ, kMasked>(t16, tbf, tdo, a, n_views, heads, stream)) return 1;
+  return launch_bwd<MODE_DKV, kMasked>(t16, tbf, tdo, a, n_views, heads, stream);
+}
+
+}  // namespace
+
+int attention_backward(const void* qkv_f16, const void* qkv_bf16, const void* d_out_bf16, const float* lse2,
+                       const float* delta, void* dqkv_bf16, int n_views, int seq, int heads, cudaStream_t stream) {
+  return run_backward<false>(qkv_f16, qkv_bf16, d_out_bf16, lse2, delta, dqkv_bf16, nullptr, 0, n_views, seq, heads, stream);
+}
+
+int attention_backward_masked(const void* qkv_f16, const void* qkv_bf16, const void* d_out_bf16, const float* lse2,
+                              const float* delta, void* dqkv_bf16, const long long* mask, int causal, int n_views, int seq,
+                              int heads, cudaStream_t stream) {
+  if (!mask && !causal)
+    return attention_backward(qkv_f16, qkv_bf16, d_out_bf16, lse2, delta, dqkv_bf16, n_views, seq, heads, stream);
+  return run_backward<true>(qkv_f16, qkv_bf16, d_out_bf16, lse2, delta, dqkv_bf16, mask, causal ? 1 : 0, n_views, seq, heads,
+                            stream);
 }
 
 }  // namespace pg

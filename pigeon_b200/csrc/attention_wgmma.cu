@@ -259,9 +259,9 @@ int attention_f16(const void* qkv, void* out, int n_views, int seq, int heads, c
 }
 
 int attention_f16_masked(const void* qkv, void* out, const long long* mask, int causal, int n_views, int seq, int heads,
-                         cudaStream_t stream) {
-  if (!mask && !causal) return attention_f16(qkv, out, n_views, seq, heads, stream);
-  return launch_attention<true>(qkv, out, n_views, seq, heads, stream, nullptr, mask, causal ? 1 : 0, "attention_masked");
+                         cudaStream_t stream, float* lse2) {
+  if (!mask && !causal) return attention_f16(qkv, out, n_views, seq, heads, stream, lse2);
+  return launch_attention<true>(qkv, out, n_views, seq, heads, stream, lse2, mask, causal ? 1 : 0, "attention_masked");
 }
 
 }  // namespace pg

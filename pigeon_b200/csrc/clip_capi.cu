@@ -17,12 +17,6 @@
 
 using namespace pg;
 
-struct pg_text {
-  pg_text_config cfg;
-  pg_text_weights w;
-  std::vector<pg_vit_layer> layers;
-};
-
 namespace {
 
 size_t text_carve(const pg_text* h, int n, int S, void* ws, float** x, void** xn, void** u) {

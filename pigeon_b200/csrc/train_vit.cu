@@ -291,7 +291,7 @@ embed_backward_kernel(const float* __restrict__ d_e, float* __restrict__ dpos, f
     float s = 0.f;
     for (int v = 0; v < n_views; ++v) s += d_e[(long)v * total + i];
     dpos[i] += s;
-    if (i < hidden) dcls[i] += s;     // token 0 is the class token
+    if (dcls && i < hidden) dcls[i] += s;     // token 0 is the class token (the text tower has none)
   }
 }
 

@@ -24,7 +24,7 @@ int attention_delta(const float* d_out, const void* out_f16, float* delta, void*
                     int num_sms, cudaStream_t stream);
 // g f32 [n_views, tokens, hidden] = d_emb [n_views, hidden] / tokens   (backward of the token mean)
 int token_mean_backward(const float* d_emb, float* g, int n_views, int tokens, int hidden, cudaStream_t stream);
-// dpos [tokens, hidden] += sum_views dE;  dcls [hidden] += sum_views dE[:, 0]
+// dpos [tokens, hidden] += sum_views dE;  dcls [hidden] (nullable) += sum_views dE[:, 0]
 int embed_backward(const float* d_e, float* dpos, float* dcls, int n_views, int tokens, int hidden, cudaStream_t stream);
 // out f32 [cols] += column sums of x [rows, ldx] (f32 | bf16)
 int column_sum_accumulate(const void* x, int src_type, long ldx, float* out, long rows, int cols, cudaStream_t stream);

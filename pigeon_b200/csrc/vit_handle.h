@@ -17,6 +17,12 @@ struct pg_vit {
   int grid_patches;
 };
 
+struct pg_text {
+  pg_text_config cfg;
+  pg_text_weights w;
+  std::vector<pg_vit_layer> layers;
+};
+
 namespace pg {
 
 int sm_count();   // cached cudaDevAttrMultiProcessorCount of the current device, -1 (and last_error) on failure

@@ -9,6 +9,7 @@
 #include <stdint.h>
 
 #include "prof.h"
+#include "text_pool.cuh"
 #include "tma_host.h"
 
 namespace pg {
@@ -202,22 +203,7 @@ __global__ void rows_layernorm_f32_kernel(const float* __restrict__ x, float* __
   const long warps = ((long)gridDim.x * blockDim.x) >> 5;
   for (long row = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
     long src = row;
-    if (ids != nullptr) {
-      const long long* ir = ids + row * S;
-      long long bv = LLONG_MIN;
-      int bt = S;
-      for (int t = lane; t < S; t += 32) {
-        const long long v = ir[t];
-        if (v > bv) { bv = v; bt = t; }   // ascending t per lane: the first maximum of the lane
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const long long ov = __shfl_xor_sync(0xffffffffu, bv, o);
-        const int ot = __shfl_xor_sync(0xffffffffu, bt, o);
-        if (ov > bv || (ov == bv && ot < bt)) { bv = ov; bt = ot; }
-      }
-      src = row * S + bt;
-    }
+    if (ids != nullptr) src = row * S + first_argmax_warp(ids + row * S, S, lane);
     float4 v[NV4];
     const float4* xr = reinterpret_cast<const float4*>(x + src * hidden);
 #pragma unroll

@@ -81,6 +81,81 @@ def attention_f16_masked(qkv: torch.Tensor, n_views: int, seq: int, heads: int, 
     return out
 
 
+def attention_f16_masked_lse(qkv: torch.Tensor, n_views: int, seq: int, heads: int, mask: torch.Tensor | None = None,
+                             causal: bool = False):
+    """`attention_f16_masked` plus lse2 f32 [n_views*heads, seq] (log2-sum-exp over the admissible keys), the side output the
+    text tower's training forward keeps for the backward pass -> (out, lse2)."""
+    if mask is not None:
+        mask = mask.to(torch.int64).contiguous()
+    _need_cuda(qkv, mask)
+    assert qkv.dtype == torch.float16 and qkv.shape == (n_views * seq, 3 * heads * 64)
+    assert mask is None or mask.shape == (n_views, seq)
+    out = torch.empty((n_views * seq, heads * 64), dtype=torch.float16, device=qkv.device)
+    lse2 = torch.empty((n_views * heads, seq), dtype=torch.float32, device=qkv.device)
+    check(load().pg_attention_f16_masked_lse(ptr(qkv), ptr(out), ptr(lse2), ptr(mask), int(bool(causal)), n_views, seq, heads,
+                                             current_stream_ptr()), "pg_attention_f16_masked_lse")
+    return out, lse2
+
+
+def attention_backward_masked(qkv: torch.Tensor, out: torch.Tensor, d_out: torch.Tensor, lse2: torch.Tensor, n_views: int,
+                              seq: int, heads: int, mask: torch.Tensor | None = None, causal: bool = False) -> torch.Tensor:
+    """Backward of `attention_f16_masked_lse`: qkv / out fp16, d_out f32 [n_views*seq, heads*64] -> dqkv bf16
+    [n_views*seq, 3*heads*64].  No mask and causal=False runs pg_attention_backward's kernels."""
+    if mask is not None:
+        mask = mask.to(torch.int64).contiguous()
+    d_out = d_out.to(torch.float32).contiguous()
+    _need_cuda(qkv, out, d_out, lse2, mask)
+    lib = load()
+    dqkv = torch.empty((n_views * seq, 3 * heads * 64), dtype=torch.bfloat16, device=qkv.device)
+    ws = torch.empty(int(lib.pg_attention_backward_workspace_bytes(n_views, seq, heads)) + 256, dtype=torch.uint8,
+                     device=qkv.device)
+    ws = ws[(-ws.data_ptr()) % 256:]
+    check(lib.pg_attention_backward_masked(ptr(qkv), ptr(out), ptr(d_out), ptr(lse2), ptr(mask), int(bool(causal)), ptr(dqkv),
+                                           n_views, seq, heads, ptr(ws), ws.numel(), current_stream_ptr()),
+          "pg_attention_backward_masked")
+    return dqkv
+
+
+def layernorm_f32(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float) -> torch.Tensor:
+    """fp32 LayerNorm over the last dim: x f32 [rows, hidden] -> f32 [rows, hidden]."""
+    _need_cuda(x, gamma, beta)
+    assert x.dtype == torch.float32
+    rows, hidden = x.reshape(-1, x.shape[-1]).shape
+    y = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    check(load().pg_layernorm_f32(ptr(x), ptr(y), ptr(gamma), ptr(beta), rows, hidden, eps, current_stream_ptr()),
+          "pg_layernorm_f32")
+    return y
+
+
+def clip_loss_grad(image_embeds: torch.Tensor, text_embeds: torch.Tensor, logit_scale: torch.Tensor,
+                   grad_scale: float = 1.0) -> dict:
+    """HF `clip_loss(logits_per_text)` and its gradient for n images and n captions: image_embeds, text_embeds f32 [n, P]
+    (not normalised), logit_scale f32 scalar CUDA tensor -> dict(loss [], d_image_embeds [n, P], d_text_embeds [n, P],
+    d_logit_scale [], logits_per_image [n, n], logits_per_text [n, n]); gradients times grad_scale."""
+    img = image_embeds.to(torch.float32).contiguous()
+    txt = text_embeds.to(torch.float32).contiguous()
+    ls = logit_scale.detach().to(torch.float32).reshape(()).contiguous()
+    _need_cuda(img, txt, ls)
+    n, P = img.shape
+    if tuple(txt.shape) != (n, P):
+        raise ValueError(f"the contrastive loss needs as many images as captions of one width (got {tuple(img.shape)} images, "
+                         f"{tuple(txt.shape)} captions)")
+    lib = load()
+    dev = img.device
+    out = dict(loss=torch.empty((), dtype=torch.float32, device=dev), d_image_embeds=torch.empty_like(img),
+               d_text_embeds=torch.empty_like(txt), d_logit_scale=torch.empty((), dtype=torch.float32, device=dev),
+               logits_per_image=torch.empty((n, n), dtype=torch.float32, device=dev),
+               logits_per_text=torch.empty((n, n), dtype=torch.float32, device=dev))
+    if n == 0:
+        return out
+    ws = torch.empty(int(lib.pg_clip_loss_grad_workspace_bytes(n, P)), dtype=torch.uint8, device=dev)
+    check(lib.pg_clip_loss_grad(ptr(img), ptr(txt), n, P, ptr(ls), float(grad_scale), ptr(ws), ws.numel(), ptr(out["loss"]),
+                                ptr(out["d_image_embeds"]), ptr(out["d_text_embeds"]), ptr(out["d_logit_scale"]),
+                                ptr(out["logits_per_image"]), ptr(out["logits_per_text"]), current_stream_ptr()),
+          "pg_clip_loss_grad")
+    return out
+
+
 def clip_project(x: torch.Tensor, w3: torch.Tensor, ln_weight: torch.Tensor | None = None,
                  ln_bias: torch.Tensor | None = None, eps: float = 1e-5) -> torch.Tensor:
     """x f32 [n, D] -> f32 [n, P] = LN(x) W^T (LN only when ln_weight / ln_bias are given), W packed by `head_pack_weight`

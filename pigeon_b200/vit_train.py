@@ -28,6 +28,48 @@ def _aligned_empty(nbytes: int, device) -> torch.Tensor:
     return raw[off:off + nbytes]
 
 
+def put_grad(p, t) -> None:
+    """p.grad += t (p.grad = a copy of t when there is none yet): gradient accumulation across backward calls."""
+    t = t.contiguous()
+    p.grad = t.clone() if p.grad is None else p.grad.add_(t)
+
+
+LAYER_GRADS = ("ln1_g", "ln1_b", "w_qkv", "b_qkv", "w_o", "b_o", "ln2_g", "ln2_b", "w_fc1", "b_fc1", "w_fc2", "b_fc2")
+
+
+def layer_grad_shapes(l: int, H: int, I: int):
+    return [(f"{l}.ln1_g", (H,)), (f"{l}.ln1_b", (H,)), (f"{l}.w_qkv", (3 * H, H)), (f"{l}.b_qkv", (3 * H,)),
+            (f"{l}.w_o", (H, H)), (f"{l}.b_o", (H,)), (f"{l}.ln2_g", (H,)), (f"{l}.ln2_b", (H,)),
+            (f"{l}.w_fc1", (I, H)), (f"{l}.b_fc1", (I,)), (f"{l}.w_fc2", (H, I)), (f"{l}.b_fc2", (H,))]
+
+
+def put_layer_grads(L, g: Dict[str, torch.Tensor], l: int, H: int) -> None:
+    """Publish the fused gradients of encoder layer l (HF CLIPEncoderLayer L) into its parameters' .grad."""
+    sa, mlp = L.self_attn, L.mlp
+    for i, proj in enumerate((sa.q_proj, sa.k_proj, sa.v_proj)):
+        put_grad(proj.weight, g[f"{l}.w_qkv"][i * H:(i + 1) * H])
+        put_grad(proj.bias, g[f"{l}.b_qkv"][i * H:(i + 1) * H])
+    put_grad(sa.out_proj.weight, g[f"{l}.w_o"]); put_grad(sa.out_proj.bias, g[f"{l}.b_o"])
+    put_grad(L.layer_norm1.weight, g[f"{l}.ln1_g"]); put_grad(L.layer_norm1.bias, g[f"{l}.ln1_b"])
+    put_grad(L.layer_norm2.weight, g[f"{l}.ln2_g"]); put_grad(L.layer_norm2.bias, g[f"{l}.ln2_b"])
+    put_grad(mlp.fc1.weight, g[f"{l}.w_fc1"]); put_grad(mlp.fc1.bias, g[f"{l}.b_fc1"])
+    put_grad(mlp.fc2.weight, g[f"{l}.w_fc2"]); put_grad(mlp.fc2.bias, g[f"{l}.b_fc2"])
+
+
+@torch.no_grad()
+def transpose_layers(layers, versions, wt: list, wt_version: dict) -> None:
+    """wt[l] = bf16 transposes of encoder layer l's four weight matrices, redone only where versions[l] moved."""
+    bf = torch.bfloat16
+    for l, L in enumerate(layers):
+        if wt[l] is not None and wt_version.get(l) == versions[l]:
+            continue
+        sa, mlp = L.self_attn, L.mlp
+        wqkv = torch.cat([sa.q_proj.weight, sa.k_proj.weight, sa.v_proj.weight], dim=0)      # [3H, H]
+        wt[l] = dict(w_qkv_t=wqkv.t().contiguous().to(bf), w_o_t=sa.out_proj.weight.t().contiguous().to(bf),
+                     w_fc1_t=mlp.fc1.weight.t().contiguous().to(bf), w_fc2_t=mlp.fc2.weight.t().contiguous().to(bf))
+        wt_version[l] = versions[l]
+
+
 class TowerTrainer:
     """Owns the activation arena, the transposed bf16 weights and the fused gradient buffers of one CLIPVisionTower."""
 
@@ -87,6 +129,8 @@ class TowerTrainer:
         saved = _lib.VitSaved()
         for name, b in top:
             setattr(saved, name, base + off)
+            if name == "x_out":
+                self._x_out_off = off
             off += _align(b)
         layers = (_lib.VitSavedLayer * d.layers)()
         for l in range(d.layers):
@@ -99,20 +143,9 @@ class TowerTrainer:
     def _transposed_weights(self):
         """bf16 transposes of the four weight matrices of every layer (B operands of the backward GEMMs); only the layers whose
         parameters moved since the last call are redone (the last one, under the reference's fine-tune policy)."""
-        versions = self.tower._group_versions()
         if self._wt is None:
             self._wt, self._wt_version = [None] * self.dims.layers, {}
-        bf = torch.bfloat16
-        with torch.no_grad():
-            for l, L in enumerate(self.tower.vision_model.encoder.layers):
-                if self._wt[l] is not None and self._wt_version.get(l) == versions[l]:
-                    continue
-                sa, mlp = L.self_attn, L.mlp
-                wqkv = torch.cat([sa.q_proj.weight, sa.k_proj.weight, sa.v_proj.weight], dim=0)      # [3H, H]
-                self._wt[l] = dict(w_qkv_t=wqkv.t().contiguous().to(bf), w_o_t=sa.out_proj.weight.t().contiguous().to(bf),
-                                   w_fc1_t=mlp.fc1.weight.t().contiguous().to(bf),
-                                   w_fc2_t=mlp.fc2.weight.t().contiguous().to(bf))
-                self._wt_version[l] = versions[l]
+        transpose_layers(self.tower.vision_model.encoder.layers, self.tower._group_versions(), self._wt, self._wt_version)
         return self._wt
 
     def _pending_grads(self):
@@ -128,9 +161,7 @@ class TowerTrainer:
         H, I = d.hidden, d.intermediate
         for l, t in enumerate(layers):
             if t:
-                shapes += [(f"{l}.ln1_g", (H,)), (f"{l}.ln1_b", (H,)), (f"{l}.w_qkv", (3 * H, H)), (f"{l}.b_qkv", (3 * H,)),
-                           (f"{l}.w_o", (H, H)), (f"{l}.b_o", (H,)), (f"{l}.ln2_g", (H,)), (f"{l}.ln2_b", (H,)),
-                           (f"{l}.w_fc1", (I, H)), (f"{l}.b_fc1", (I,)), (f"{l}.w_fc2", (H, I)), (f"{l}.b_fc2", (H,))]
+                shapes += layer_grad_shapes(l, H, I)
         # ONE flat fp32 buffer (every tensor 16-byte aligned inside it): a single all-reduce averages the whole tower
         offs, total = [], 0
         for _, shp in shapes:
@@ -179,6 +210,16 @@ class TowerTrainer:
             out.append((d.layers, off(g["patch_w"]), off(g["pre_ln_b"]) + g["pre_ln_b"].numel()))
         return out
 
+    def cls_rows(self) -> torch.Tensor:
+        """last_hidden_state[:, 0] of the views of the last forward, f32 [n, hidden] (a copy out of the arena): the CLS rows
+        that CLIPModel feeds to post_layernorm and visual_projection."""
+        if self._saved is None:
+            raise PigeonB200Error("cls_rows() needs a preceding forward()")
+        d, n = self.dims, self._saved_views
+        nbytes = n * d.tokens * d.hidden * 4
+        x = self._arena[self._x_out_off:self._x_out_off + nbytes].view(torch.float32).view(n, d.tokens, d.hidden)
+        return x[:, 0].contiguous()
+
     @torch.no_grad()
     def backward(self, d_emb: torch.Tensor, overlap_world: int = 1) -> None:
         """d_emb f32 [n, hidden] for the views of the last forward; gradients accumulate in the pending buffers.
@@ -186,6 +227,15 @@ class TowerTrainer:
         overlap_world > 1 (the LAST chunk of a micro-batch under torch.distributed): each layer's gradient bucket is summed
         over the ranks by an NCCL all-reduce on a side stream as soon as pg_vit_backward reports the layer done, while the
         layers below are still in their backward; `finalize` then only waits for the outstanding buckets."""
+        self._backward(d_emb, "pg_vit_backward", overlap_world)
+
+    @torch.no_grad()
+    def backward_cls(self, d_cls: torch.Tensor) -> None:
+        """d_cls f32 [n, hidden]: gradient of the CLS rows (`cls_rows()`) of the views of the last forward (pg_vit_backward_cls);
+        gradients accumulate in the pending buffers."""
+        self._backward(d_cls, "pg_vit_backward_cls", 1)
+
+    def _backward(self, d_emb: torch.Tensor, entry: str, overlap_world: int) -> None:
         d = self.dims
         n = self._saved_views
         if self._saved is None or d_emb.shape != (n, d.hidden):
@@ -200,7 +250,7 @@ class TowerTrainer:
             for k, t in wt[l].items():
                 setattr(lb[l], k, t.data_ptr())
             if layers[l]:
-                for k in ("ln1_g", "ln1_b", "w_qkv", "b_qkv", "w_o", "b_o", "ln2_g", "ln2_b", "w_fc1", "b_fc1", "w_fc2", "b_fc2"):
+                for k in LAYER_GRADS:
                     setattr(lb[l], "d_" + k, g[f"{l}.{k}"].data_ptr())
         grads = _lib.VitGrads()
         if emb_train:
@@ -221,8 +271,8 @@ class TowerTrainer:
         if self._ws is None or self._ws.numel() < need:
             self._ws = None
             self._ws = _aligned_empty(need, d_emb.device)
-        check(self._lib.pg_vit_backward(eng._handle, C.byref(self._saved), ptr(d_emb), n, C.byref(grads), ptr(self._ws),
-                                        self._ws.numel(), current_stream_ptr()), "pg_vit_backward")
+        check(getattr(self._lib, entry)(eng._handle, C.byref(self._saved), ptr(d_emb), n, C.byref(grads), ptr(self._ws),
+                                        self._ws.numel(), current_stream_ptr()), entry)
         if overlap_world > 1:
             self._works = []
             with torch.cuda.stream(self._side):
@@ -245,11 +295,7 @@ class TowerTrainer:
                 torch.distributed.all_reduce(self._pending_flat)
             self._pending_flat.mul_(1.0 / world)
         vm = self.tower.vision_model
-
-        def put(p, t):
-            t = t.contiguous()
-            p.grad = t.clone() if p.grad is None else p.grad.add_(t)
-
+        put = put_grad
         if "patch_w" in g:
             e = vm.embeddings
             put(e.patch_embedding.weight, g["patch_w"][:, : d.patch_k].reshape(e.patch_embedding.weight.shape))
@@ -257,17 +303,7 @@ class TowerTrainer:
             put(e.position_embedding.weight, g["pos_emb"])
             put(vm.pre_layrnorm.weight, g["pre_ln_g"])
             put(vm.pre_layrnorm.bias, g["pre_ln_b"])
-        H = d.hidden
         for l, L in enumerate(vm.encoder.layers):
-            if f"{l}.w_qkv" not in g:
-                continue
-            sa, mlp = L.self_attn, L.mlp
-            for i, proj in enumerate((sa.q_proj, sa.k_proj, sa.v_proj)):
-                put(proj.weight, g[f"{l}.w_qkv"][i * H:(i + 1) * H])
-                put(proj.bias, g[f"{l}.b_qkv"][i * H:(i + 1) * H])
-            put(sa.out_proj.weight, g[f"{l}.w_o"]); put(sa.out_proj.bias, g[f"{l}.b_o"])
-            put(L.layer_norm1.weight, g[f"{l}.ln1_g"]); put(L.layer_norm1.bias, g[f"{l}.ln1_b"])
-            put(L.layer_norm2.weight, g[f"{l}.ln2_g"]); put(L.layer_norm2.bias, g[f"{l}.ln2_b"])
-            put(mlp.fc1.weight, g[f"{l}.w_fc1"]); put(mlp.fc1.bias, g[f"{l}.b_fc1"])
-            put(mlp.fc2.weight, g[f"{l}.w_fc2"]); put(mlp.fc2.bias, g[f"{l}.b_fc2"])
+            if f"{l}.w_qkv" in g:
+                put_layer_grads(L, g, l, d.hidden)
         self._pending = None
