@@ -22,6 +22,7 @@ OBJ_DIR = CSRC / "build"
 SOURCES = [
     "tma_host.cu",
     "gemm_wgmma.cu",
+    "gemm_pingpong.cu",
     "attention_wgmma.cu",
     "nccl_gather.cu",
     "vit_misc.cu",

@@ -157,6 +157,7 @@ SIGNATURES = {
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pg_refiner_set_schedule": (c_int32, [c_int32]),
     "pg_head_set_fused": (c_int32, [c_int32]),
+    "pg_gemm_set_schedule": (c_int32, [c_int32]),
     "pg_refiner_bank_sqnorm": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p]),
     "pg_refiner_scan": (c_int32, [C.POINTER(RefinerBank), c_void_p, c_int64, c_int32, c_void_p, c_int32, c_int32, c_void_p,
                                   c_size_t, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -525,6 +525,8 @@ int pg_gemm_f16(const void* a, int32_t lda, const void* w, int32_t ldw, void* ou
   return gemm_f16(p, sms, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pg_gemm_set_schedule(int32_t mode) { return gemm_set_schedule(mode); }
+
 int pg_layernorm_f16(const float* x, void* y, const float* gamma, const float* beta, int64_t rows, int32_t hidden,
                      float eps, void* stream) {
   if (!x || !y || !gamma || !beta) { set_last_error("pg_layernorm_f16: null argument"); return 1; }

@@ -15,15 +15,40 @@
 //               (each warp 32 rows: bias / activation / residual -> global)
 //   warp 4      TMA producer (one lane): global -> 4-stage smem ring, 128B swizzle; it runs ahead into the next tile
 //               while the warpgroup is in its epilogue
+// K-major problems run the ping-pong kernel of gemm_pingpong.cu (same tiles and MMAs, two consumer warpgroups) unless
+// pg_gemm_set_schedule(1) selects this one; MN-major operands always run here.  launch<EPI> below checks the problem and
+// builds the tensor maps for both.
 #include "gemm.h"
 #include "gemm_epilogue.cuh"
+#include "gemm_pingpong.h"
 #include "ptx.cuh"
 #include "prof.h"
 #include "tma_host.h"
 
 #include <atomic>
+#include <cstdlib>
 
 namespace pg {
+
+// Process-wide kernel choice (pg_gemm_set_schedule).  It exists so that tests can take the single-warpgroup kernel as the
+// bit-exact reference of the ping-pong kernel and a benchmark can compare the two in one process; it is not a tuning knob.
+// PG_GEMM_SCHEDULE=1 only sets the initial value, once.
+static std::atomic<int> g_gemm_schedule{-1};
+static int gemm_schedule() {
+  int v = g_gemm_schedule.load(std::memory_order_relaxed);
+  if (v < 0) {
+    const char* e = getenv("PG_GEMM_SCHEDULE");
+    v = (e && e[0] == '1') ? 1 : 0;
+    g_gemm_schedule.store(v, std::memory_order_relaxed);
+  }
+  return v;
+}
+
+int gemm_set_schedule(int mode) {
+  if (mode != 0 && mode != 1) { set_last_error("pg_gemm_set_schedule: mode %d not in {0, 1}", mode); return 1; }
+  g_gemm_schedule.store(mode, std::memory_order_relaxed);
+  return 0;
+}
 
 namespace {
 
@@ -162,10 +187,6 @@ int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& 
     if (e != cudaSuccess) { set_last_error("gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return 1; }
     attr_set[dev].store(1, std::memory_order_release);
   }
-  static const char* const kNames[] = {"gemm_f16_bias", "gemm_f16_bias_qgelu", "gemm_f32_bias_resid", "gemm_f32_bias", "gemm_f32_rowmap",
-                                       "gemm_bf16_dgelu", "gemm_f16_bias_qgelu_save", "gemm_f32_bias_resid_stats", "gemm_f16_ln_bias",
-                                       "gemm_f16_ln_bias_qgelu"};
-  ProfScope prof(kNames[EPI], stream);
   kern<<<grid, kNumThreads, kSmemBytes, stream>>>(ta, tb, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error("gemm launch: %s", cudaGetErrorString(e)); return 1; }
@@ -209,6 +230,13 @@ int launch(const GemmProblem& p, int num_sms, cudaStream_t stream) {
   const int m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M, n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int tiles = m_blocks * n_blocks;
   const int grid = tiles < num_sms ? tiles : num_sms;
+  static const char* const kNames[] = {"gemm_f16_bias", "gemm_f16_bias_qgelu", "gemm_f32_bias_resid", "gemm_f32_bias", "gemm_f32_rowmap",
+                                       "gemm_bf16_dgelu", "gemm_f16_bias_qgelu_save", "gemm_f32_bias_resid_stats", "gemm_f16_ln_bias",
+                                       "gemm_f16_ln_bias_qgelu"};
+  ProfScope prof(kNames[EPI], stream);
+  // K-major problems go to the ping-pong kernel (gemm_pingpong.cu): same tiles and MMAs, so the same bits, with each
+  // tile's epilogue overlapping the next tile's MMAs.  MN-major operands (pg_gemm_tn) stay on gemm_f16_kernel.
+  if (!p.mn_major && gemm_schedule() == 0) return gemm_pingpong_launch(EPI, p.operand_bf16 != 0, ta, tb, a, grid, stream);
   if (p.mn_major) return p.operand_bf16 ? launch_kernel<EPI, true, true>(ta, tb, a, grid, stream) : launch_kernel<EPI, false, true>(ta, tb, a, grid, stream);
   return p.operand_bf16 ? launch_kernel<EPI, true, false>(ta, tb, a, grid, stream) : launch_kernel<EPI, false, false>(ta, tb, a, grid, stream);
 }

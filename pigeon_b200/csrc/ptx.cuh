@@ -182,6 +182,25 @@ template <int ID>
 __device__ __forceinline__ void named_barrier(int threads) {
   asm volatile("bar.sync %0, %1;" ::"n"(ID), "r"(threads) : "memory");
 }
+// The same with a run-time barrier id, and its non-blocking half: bar.arrive counts the caller towards `threads` without
+// waiting (producer side of a producer / consumer hand-off between warpgroups).
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_barrier_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// Per-warpgroup register budget (all 128 threads of the warpgroup execute it): dec releases registers to the SM's pool,
+// inc waits until it can take them.  N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 // fp32 pair FMA: two independent fused multiply-adds (sm_90 has no packed-fp32 instruction).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {

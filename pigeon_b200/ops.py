@@ -34,6 +34,11 @@ def gemm_f16(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, epilog
     return out
 
 
+def gemm_set_schedule(mode: int) -> None:
+    """Kernel of every K-major GEMM, process-wide: 0 = automatic (ping-pong), 1 = the single-warpgroup kernel (same bits)."""
+    check(load().pg_gemm_set_schedule(int(mode)), "pg_gemm_set_schedule")
+
+
 def layernorm_f16(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float) -> torch.Tensor:
     _need_cuda(x, gamma, beta)
     assert x.dtype == torch.float32
