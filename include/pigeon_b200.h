@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define PG_ABI_VERSION 3
+#define PG_ABI_VERSION 4
 
 /* ---------------------------------------------------------------------------------------------------
  * Library
@@ -418,7 +418,16 @@ enum {
   PG_EPI_F16_BIAS = 0,       /* out fp16 = A W^T + bias                       (q/k/v projection) */
   PG_EPI_F16_BIAS_QGELU = 1, /* out fp16 = quick_gelu(A W^T + bias)            (mlp.fc1)          */
   PG_EPI_F32_BIAS_RESID = 2, /* out f32 += A W^T + bias                        (out_proj, mlp.fc2) */
-  PG_EPI_F32_BIAS = 3        /* out f32 = A W^T + bias (bias may be NULL)                          */
+  PG_EPI_F32_BIAS = 3,       /* out f32 = A W^T + bias (bias may be NULL)                          */
+  /* the remaining epilogues are reached only through pg_gemm_problem_run (the towers use them internally) */
+  PG_EPI_F32_ROWMAP = 4,     /* out f32 [mul * (r / div) + r % div + add] = A W^T + bias   (patch embedding -> token rows) */
+  PG_EPI_BF16_DGELU = 5,     /* out bf16 = (A W^T) * quick_gelu'(aux fp16)                  (backward through mlp.fc1's activation) */
+  PG_EPI_F16_BIAS_QGELU_SAVE = 6,  /* out fp16 = quick_gelu(A W^T + bias), aux fp16 = A W^T + bias  (training forward of mlp.fc1) */
+  PG_EPI_F32_BIAS_RESID_STATS = 7, /* PG_EPI_F32_BIAS_RESID, aux fp16 = the new residual row, stats[r][c / 128] = (sum, sum of squares)
+                                      of those fp16 values over 128 columns   (LayerNorm producer: out_proj, fc2) */
+  PG_EPI_F16_LN_BIAS = 8,    /* out fp16 = rstd * (A W^T - mu * colsum) + bias, (mu, rstd) of row r of A from stats [M, K / 128]
+                                (LayerNorm consumer: qkv; W = gamma-scaled weight, bias = b + W beta, colsum = row sums of W) */
+  PG_EPI_F16_LN_BIAS_QGELU = 9     /* quick_gelu of the same                                    (LayerNorm consumer: fc1) */
 };
 /* D[M,N] = A[M,K] (fp16, row stride lda) * W[N,K]^T (fp16, row stride ldw), fp32 accumulate on wgmma. */
 int pg_gemm_f16(const void* a, int32_t lda, const void* w, int32_t ldw, void* out, int32_t ldo, const float* bias,
@@ -437,6 +446,31 @@ int pg_gemm_ex(const void* a, int32_t lda, const void* w, int32_t ldw, void* out
  * M > 128, N % 256 == 0, lda and ldw multiples of 8 (other shapes are rejected); epilogue PG_EPI_F32_BIAS (overwrite) or PG_EPI_F32_BIAS_RESID (accumulate in place). */
 int pg_gemm_tn(const void* a, int32_t lda, const void* w, int32_t ldw, float* out, int32_t ldo, int32_t M, int32_t N,
                int32_t K, int32_t accumulate, int32_t operand_bf16, void* stream);
+/* The whole GEMM problem, every epilogue (pg_gemm_f16 / pg_gemm_ex / pg_gemm_tn fill a subset of it).  Pointers as in
+ * pg_gemm_ex; aux fp16 [M, ldo] for epilogues 5-7 (16-byte aligned); stats float2 (8-byte aligned) [M, N / 128] written by 7,
+ * [M, K / 128] read by 8 and 9; colsum f32 [N] (16-byte aligned) and ln_eps for 8 and 9; rowmap_* for 4 (div <= 0 means 1);
+ * mn_major != 0 selects pg_gemm_tn's operand layout (a [K, lda], w [K, ldw]).  Shapes an epilogue does not take are rejected
+ * before anything is enqueued. */
+typedef struct pg_gemm_problem {
+  int32_t M, N, K;
+  const void* a;
+  int32_t lda;
+  const void* w;
+  int32_t ldw;
+  void* out;
+  int32_t ldo;
+  const float* bias;
+  int32_t epilogue;
+  int32_t rowmap_div, rowmap_mul, rowmap_add;
+  int32_t operand_bf16;
+  const float* resid;
+  void* aux;
+  int32_t mn_major;
+  float* stats;
+  const float* colsum;
+  float ln_eps;
+} pg_gemm_problem;
+int pg_gemm_problem_run(const pg_gemm_problem* p, void* stream);
 /* LayerNorm over the last dim: x f32 [rows, hidden] -> y fp16 [rows, hidden]. */
 int pg_layernorm_f16(const float* x, void* y, const float* gamma, const float* beta, int64_t rows, int32_t hidden,
                      float eps, void* stream);

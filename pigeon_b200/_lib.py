@@ -83,6 +83,14 @@ class RefinerBank(C.Structure):
                 ("member_idx", c_void_p), ("data_emb", c_void_p), ("data_lnglat", c_void_p), ("proto_sqnorm", c_void_p), ("num_protos", c_int64), ("live_cells", c_int32)]
 
 
+class GemmProblem(C.Structure):
+    _fields_ = [("M", c_int32), ("N", c_int32), ("K", c_int32), ("a", c_void_p), ("lda", c_int32), ("w", c_void_p),
+                ("ldw", c_int32), ("out", c_void_p), ("ldo", c_int32), ("bias", c_void_p), ("epilogue", c_int32),
+                ("rowmap_div", c_int32), ("rowmap_mul", c_int32), ("rowmap_add", c_int32), ("operand_bf16", c_int32),
+                ("resid", c_void_p), ("aux", c_void_p), ("mn_major", c_int32), ("stats", c_void_p), ("colsum", c_void_p),
+                ("ln_eps", c_float)]
+
+
 # name -> (restype, argtypes); must list every symbol declared in include/pigeon_b200.h
 SIGNATURES = {
     "pg_abi_version": (c_int32, []),
@@ -127,6 +135,7 @@ SIGNATURES = {
                              c_int32, c_int32, c_int32, c_void_p]),
     "pg_gemm_tn": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                              c_void_p]),
+    "pg_gemm_problem_run": (c_int32, [C.POINTER(GemmProblem), c_void_p]),
     "pg_attention_f16_lse": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
     "pg_attention_backward_workspace_bytes": (c_size_t, [c_int32, c_int32, c_int32]),
     "pg_attention_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
@@ -180,9 +189,11 @@ SIGNATURES = {
                                            c_void_p]),
 }
 
-ABI_VERSION = 3   # == PG_ABI_VERSION in include/pigeon_b200.h; bumped whenever a signature or struct changes
+ABI_VERSION = 4   # == PG_ABI_VERSION in include/pigeon_b200.h; bumped whenever a signature or struct changes
 
 EPI_F16_BIAS, EPI_F16_BIAS_QGELU, EPI_F32_BIAS_RESID, EPI_F32_BIAS = 0, 1, 2, 3
+EPI_F32_ROWMAP, EPI_BF16_DGELU, EPI_F16_BIAS_QGELU_SAVE, EPI_F32_BIAS_RESID_STATS, EPI_F16_LN_BIAS, EPI_F16_LN_BIAS_QGELU = \
+    4, 5, 6, 7, 8, 9
 
 _lib: Optional[C.CDLL] = None
 

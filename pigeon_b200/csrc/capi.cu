@@ -527,6 +527,24 @@ int pg_gemm_f16(const void* a, int32_t lda, const void* w, int32_t ldw, void* ou
 
 int pg_gemm_set_schedule(int32_t mode) { return gemm_set_schedule(mode); }
 
+static_assert(PG_EPI_F16_BIAS == EPI_F16_BIAS && PG_EPI_F32_BIAS == EPI_F32_BIAS && PG_EPI_F32_ROWMAP == EPI_F32_ROWMAP &&
+              PG_EPI_BF16_DGELU == EPI_BF16_DGELU && PG_EPI_F16_BIAS_QGELU_SAVE == EPI_F16_BIAS_QGELU_SAVE &&
+              PG_EPI_F32_BIAS_RESID_STATS == EPI_F32_BIAS_RESID_STATS && PG_EPI_F16_LN_BIAS == EPI_F16_LN_BIAS &&
+              PG_EPI_F16_LN_BIAS_QGELU == EPI_F16_LN_BIAS_QGELU, "PG_EPI_* mirror pg::GemmEpilogue");
+
+int pg_gemm_problem_run(const pg_gemm_problem* q, void* stream) {
+  if (!q || !q->a || !q->w || !q->out) { set_last_error("pg_gemm_problem_run: null argument"); return 1; }
+  const int sms = sm_count();
+  if (sms < 0) return 1;
+  GemmProblem p{};
+  p.M = q->M; p.N = q->N; p.K = q->K; p.a = q->a; p.lda = q->lda; p.w = q->w; p.ldw = q->ldw; p.out = q->out; p.ldo = q->ldo;
+  p.bias = q->bias; p.epi = q->epilogue;
+  p.rowmap_div = q->rowmap_div; p.rowmap_mul = q->rowmap_mul; p.rowmap_add = q->rowmap_add;
+  p.operand_bf16 = q->operand_bf16 ? 1 : 0; p.resid = q->resid; p.aux = q->aux; p.mn_major = q->mn_major ? 1 : 0;
+  p.stats = q->stats; p.colsum = q->colsum; p.ln_eps = q->ln_eps;
+  return gemm_f16(p, sms, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int pg_layernorm_f16(const float* x, void* y, const float* gamma, const float* beta, int64_t rows, int32_t hidden,
                      float eps, void* stream) {
   if (!x || !y || !gamma || !beta) { set_last_error("pg_layernorm_f16: null argument"); return 1; }

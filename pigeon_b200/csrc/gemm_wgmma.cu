@@ -250,6 +250,18 @@ int gemm_f16(const GemmProblem& p, int num_sms, cudaStream_t stream) {
        reinterpret_cast<uintptr_t>(p.bias)) & 15) {
     set_last_error("gemm: pointers must be 16-byte aligned"); return 1;
   }
+  // the epilogues read the residual with 16-byte and the LayerNorm moments with 8-byte vector accesses
+  if (reinterpret_cast<uintptr_t>(p.resid) & 15) { set_last_error("gemm: resid must be 16-byte aligned"); return 1; }
+  if ((p.epi == EPI_F32_BIAS_RESID_STATS || p.epi == EPI_F16_LN_BIAS || p.epi == EPI_F16_LN_BIAS_QGELU) &&
+      (reinterpret_cast<uintptr_t>(p.stats) & 7)) {
+    set_last_error("gemm: stats must be 8-byte aligned"); return 1;
+  }
+  if (p.ldo < p.N) { set_last_error("gemm: ldo %d < N %d", p.ldo, p.N); return 1; }
+  if (p.mn_major ? (p.lda < p.M || p.ldw < p.N) : (p.lda < p.K || p.ldw < p.K)) {
+    set_last_error("gemm: lda %d / ldw %d shorter than the rows they stride (%s)", p.lda, p.ldw,
+                   p.mn_major ? "MN-major: lda >= M, ldw >= N" : "lda >= K, ldw >= K");
+    return 1;
+  }
   if (num_sms < 1) num_sms = 1;
   // The weight-gradient form takes the shapes pg_gemm_tn documents; its callers transpose and use the K-major form otherwise.
   if (p.mn_major && !(p.N % 256 == 0 && p.M > 128)) { set_last_error("gemm: MN-major operands need N %% 256 == 0 and M > 128"); return 1; }

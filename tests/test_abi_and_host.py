@@ -409,9 +409,10 @@ def test_docs_only_name_entry_points_that_exist():
         assert not unknown, (doc, sorted(unknown))
 
 
-def test_ctypes_structs_match_the_header_layout(tmp_path):
-    """Every ctypes mirror in pigeon_b200/_lib.py has the size and the field offsets gcc computes from include/pigeon_b200.h
-    (a reordered, missing or mistyped field would silently corrupt the arguments of the C ABI)."""
+def test_ctypes_structs_match_the_header_layout_at_abi_4(tmp_path):
+    """Every ctypes mirror in pigeon_b200/_lib.py, pg_gemm_problem included, has the size and the field offsets gcc computes
+    from include/pigeon_b200.h (a reordered, missing or mistyped field would silently corrupt the arguments of the C ABI), and
+    the binding is at ABI version 4, the first with pg_gemm_problem."""
     import ctypes as C
     import shutil
     import subprocess
@@ -421,7 +422,8 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
         pytest.skip("gcc not available")
     pairs = {"pg_vit_config": _lib.VitConfig, "pg_image": _lib.Image, "pg_vit_layer": _lib.VitLayer,
              "pg_vit_saved_layer": _lib.VitSavedLayer, "pg_vit_saved": _lib.VitSaved, "pg_vit_layer_bwd": _lib.VitLayerBwd,
-             "pg_vit_grads": _lib.VitGrads, "pg_vit_weights": _lib.VitWeights, "pg_refiner_bank": _lib.RefinerBank}
+             "pg_vit_grads": _lib.VitGrads, "pg_vit_weights": _lib.VitWeights, "pg_refiner_bank": _lib.RefinerBank,
+             "pg_gemm_problem": _lib.GemmProblem}
     lines = ["#include <stddef.h>", "#include <stdio.h>", '#include "pigeon_b200.h"', "int main(void) {"]
     for cname, cls in pairs.items():
         lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
@@ -440,4 +442,4 @@ def test_ctypes_structs_match_the_header_layout(tmp_path):
         assert int(got[cname]) == C.sizeof(cls), (cname, got[cname], C.sizeof(cls))
         for fname, _ in cls._fields_:
             assert int(got[f"{cname}.{fname}"]) == getattr(cls, fname).offset, (cname, fname)
-    assert _lib.ABI_VERSION == 3
+    assert _lib.ABI_VERSION == 4
