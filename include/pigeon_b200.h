@@ -217,6 +217,27 @@ int pg_adamw_step(float* param, const float* grad, float* exp_avg, float* exp_av
                   void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * CLIP pretraining optimizer step: what the HF Trainer (transformers 4.23.1, optim="adamw_hf") of reference
+ * training/train_modes.py:30-64 runs after the accumulated micro-batches.
+ * ------------------------------------------------------------------------------------------------- */
+/* Bytes of workspace pg_grad_norm_clip needs for n gradient elements. */
+size_t pg_grad_norm_clip_workspace_bytes(int64_t n);
+/* torch.nn.utils.clip_grad_norm_(params, max_norm) over one flat fp32 gradient read as grad * grad_scale: writes the device
+ * floats total_norm = ||grad * grad_scale||_2 and clip_coef = min(max_norm / (total_norm + 1e-6), 1); the gradient itself is
+ * not modified (pg_adamw_hf_step applies clip_coef).  Deterministic: the same n and bits give the same result on every run.
+ * A non-finite norm is not an error and the step is not skipped (as in torch with error_if_nonfinite=False): an inf norm
+ * gives clip_coef 0 and a NaN norm a NaN clip_coef, so the parameters the next update touches become NaN. */
+int pg_grad_norm_clip(const float* grad, int64_t n, double grad_scale, double max_norm, float* total_norm, float* clip_coef,
+                      void* workspace, size_t workspace_bytes, void* stream);
+/* transformers.optimization.AdamW.step (4.23.1, correct_bias = True) on a flat fp32 parameter, `step` counts from 1:
+ *   g = grad * grad_scale * (*clip_coef);  m = m*beta1 + (1-beta1)*g;  v = v*beta2 + (1-beta2)*g*g;
+ *   p -= lr * sqrt(1-beta2^t) / (1-beta1^t) * m / (sqrt(v) + eps);  then p += (-lr*weight_decay) * p if weight_decay > 0.
+ * clip_coef is a device pointer (NULL = 1), so the step needs no host synchronisation. */
+int pg_adamw_hf_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, double lr,
+                     double beta1, double beta2, double eps, double weight_decay, int64_t step, double grad_scale,
+                     const float* clip_coef, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Fine-tune step, vision tower ("next" row N1): the forward of pg_vit_forward with every activation the backward
  * needs kept in caller-provided buffers, and the backward itself — what autograd runs through HF
  * CLIPVisionTransformer for `accelerator.backward(output.loss)` in reference training/train_eval_loop.py:216.

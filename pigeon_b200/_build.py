@@ -38,6 +38,7 @@ SOURCES = [
     "clip.cu",
     "clip_capi.cu",
     "clip_train.cu",
+    "pretrain.cu",
 ]
 
 NVCC_FLAGS = [

@@ -160,6 +160,10 @@ SIGNATURES = {
                                    c_void_p, c_void_p]),
     "pg_adamw_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_double, c_double, c_double, c_double,
                                 c_double, c_int64, c_double, c_void_p]),
+    "pg_grad_norm_clip_workspace_bytes": (c_size_t, [c_int64]),
+    "pg_grad_norm_clip": (c_int32, [c_void_p, c_int64, c_double, c_double, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "pg_adamw_hf_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_double, c_double, c_double, c_double,
+                                   c_double, c_int64, c_double, c_void_p, c_void_p]),
     "pg_refiner_workspace_bytes": (c_size_t, [c_int64, c_int32, c_int32, c_int32]),
     "pg_refiner_forward": (c_int32, [C.POINTER(RefinerBank), c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p,
                                      c_int32, c_int32, c_float, c_double, c_void_p, c_size_t, c_void_p, c_void_p,

@@ -6,8 +6,8 @@ training/train_modes.py:30-64 pretrains into StreetCLIP and that `PretrainDatase
 Parameter names are HF's (`text_model.*`, `vision_model.*`, `visual_projection.weight`, `text_projection.weight`,
 `logit_scale`), so CLIPModel checkpoints load by name.
 
-`forward_train` + `backward` is one contrastive training step (the gradient of `clip_loss` for every parameter, for
-`training.AdamW`); the HF Trainer around it (schedule, clipping, checkpoints) is not implemented.
+`forward_train` + `backward` is one contrastive training step (the gradient of `clip_loss` for every parameter);
+`pretrain.CLIPPretrainer` is the HF Trainer loop around it (schedule, clipping, HF AdamW, checkpoints).
 
     image features = visual_projection(post_layernorm(last_hidden_state[:, 0]))      (CLS row; pg_vit_forward_cls)
     text features  = text_projection(pooled)                                          (pg_text_forward)
@@ -92,6 +92,58 @@ class CLIPModel(nn.Module):
         missing, unexpected = model.load_state_dict(sd, strict=False)
         if missing or unexpected:
             raise PigeonB200Error(f"cannot map HF weights: missing={missing} unexpected={unexpected}")
+        return model
+
+    def hf_config_dict(self) -> dict:
+        """The `config.json` of an HF CLIPModel with this geometry (quick-GELU towers; BOS / EOS are the last two ids, as in
+        CLIP's tokenizer, so HF pools the first EOS row where this model pools the first row of the largest id)."""
+        t, v = self.text_dims, self.vision_dims
+        return dict(
+            architectures=["CLIPModel"], model_type="clip", projection_dim=self.projection_dim,
+            logit_scale_init_value=LOGIT_SCALE_INIT, initializer_factor=1.0,
+            text_config=dict(model_type="clip_text_model", vocab_size=t.vocab, max_position_embeddings=t.max_positions,
+                             hidden_size=t.hidden, num_attention_heads=t.heads, intermediate_size=t.intermediate,
+                             num_hidden_layers=t.layers, layer_norm_eps=t.ln_eps, hidden_act="quick_gelu",
+                             projection_dim=self.projection_dim, pad_token_id=1, bos_token_id=t.vocab - 2,
+                             eos_token_id=t.vocab - 1),
+            vision_config=dict(model_type="clip_vision_model", image_size=v.image_size, patch_size=v.patch_size,
+                               hidden_size=v.hidden, num_attention_heads=v.heads, intermediate_size=v.intermediate,
+                               num_hidden_layers=v.layers, layer_norm_eps=v.ln_eps, hidden_act="quick_gelu",
+                               projection_dim=self.projection_dim, num_channels=3))
+
+    def save_pretrained(self, directory: str) -> None:
+        """`pytorch_model.bin` (HF parameter names, fp32 on the CPU) and `config.json`: a directory that
+        `transformers.CLIPModel.from_pretrained` and `CLIPModel.from_pretrained` both load."""
+        import json
+        import os
+        os.makedirs(directory, exist_ok=True)
+        torch.save({k: v.detach().cpu().clone() for k, v in self.state_dict().items()},
+                   os.path.join(directory, "pytorch_model.bin"))
+        with open(os.path.join(directory, "config.json"), "w") as f:
+            json.dump(self.hf_config_dict(), f, indent=2, sort_keys=True)
+
+    @classmethod
+    def from_pretrained(cls, name_or_path: str) -> "CLIPModel":
+        """A directory with `config.json` and `pytorch_model.bin` (written by `save_pretrained`, an HF Trainer checkpoint or
+        `transformers.CLIPModel.save_pretrained(..., safe_serialization=False)`), else an HF model name or a directory
+        that `transformers.CLIPModel.from_pretrained` loads (through `from_hf`).  The model stays on the CPU."""
+        import json
+        import os
+        from types import SimpleNamespace
+        cfg_path, bin_path = os.path.join(name_or_path, "config.json"), os.path.join(name_or_path, "pytorch_model.bin")
+        if not (os.path.isfile(cfg_path) and os.path.isfile(bin_path)):
+            from transformers import CLIPModel as HFCLIPModel
+            return cls.from_hf(HFCLIPModel.from_pretrained(name_or_path))
+        with open(cfg_path) as f:
+            cfg = json.load(f)
+        model = cls(TextDims.from_hf_config(SimpleNamespace(**{"layer_norm_eps": 1e-5, **cfg["text_config"]})),
+                    VitDims.from_hf_config(SimpleNamespace(**{"layer_norm_eps": 1e-5, **cfg["vision_config"]})),
+                    projection_dim=cfg["projection_dim"])
+        sd = torch.load(bin_path, map_location="cpu", weights_only=True)
+        sd = {k: v for k, v in sd.items() if "position_ids" not in k}
+        missing, unexpected = model.load_state_dict(sd, strict=False)
+        if missing or unexpected:
+            raise PigeonB200Error(f"cannot map checkpoint weights: missing={missing} unexpected={unexpected}")
         return model
 
     # ------------------------------------------------------------------------------------------ kernels

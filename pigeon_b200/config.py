@@ -42,3 +42,20 @@ EVAL_BATCH_SIZE = 256
 TRAIN_ARGS = SimpleNamespace(output_dir='saved_models', per_device_train_batch_size=256, per_device_eval_batch_size=256,
                              num_train_epochs=1000, learning_rate=2e-5, logging_steps=1, gradient_accumulation_steps=1,
                              seed=330)
+
+# Pretraining arguments (the HF TrainingArguments fields `pretrain.CLIPPretrainer` reads; report_to='tensorboard' is not
+# implemented: the log goes to trainer_state.json and the `pretrain` logger)
+_PRETRAIN_COMMON = dict(overwrite_output_dir=True, do_train=True, do_eval=True, evaluation_strategy='steps', eval_steps=50,
+                        per_device_train_batch_size=32, per_device_eval_batch_size=32, gradient_accumulation_steps=8,
+                        weight_decay=0.001, adam_beta1=0.9, adam_beta2=0.98, adam_epsilon=1e-06, max_grad_norm=1.0,
+                        max_steps=-1, lr_scheduler_type='linear', logging_first_step=False, logging_strategy='steps',
+                        logging_steps=1, save_strategy='steps', save_steps=50, seed=42, dataloader_drop_last=True,
+                        run_name=None, adafactor=False, report_to='tensorboard', skip_memory_metrics=True,
+                        resume_from_checkpoint=None, warmup_steps=0)
+
+# PIGEOTTO                                                             (config.py:112-143)
+PRETAIN_ARGS_YFCC = SimpleNamespace(**_PRETRAIN_COMMON, output_dir='saved_models/pretrained_yfcc', learning_rate=5e-07,
+                                    num_train_epochs=4, warmup_ratio=0.02)
+# PIGEON                                                               (config.py:145-177)
+PRETAIN_ARGS = SimpleNamespace(**_PRETRAIN_COMMON, output_dir='saved_models/pretrained', learning_rate=1e-06,
+                               num_train_epochs=20, warmup_ratio=0.2)

@@ -15,6 +15,7 @@
 #include "gemm.h"
 #include "head.h"
 #include "preprocess.h"
+#include "pretrain.h"
 #include "refiner.h"
 #include "tma_host.h"
 #include "train.h"
@@ -332,6 +333,30 @@ int pg_adamw_step(float* param, const float* grad, float* exp_avg, float* exp_av
   }
   return adamw_step(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale,
                     reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------- CLIP pretraining step
+size_t pg_grad_norm_clip_workspace_bytes(int64_t n) { return grad_norm_clip_workspace_bytes(n); }
+
+int pg_grad_norm_clip(const float* grad, int64_t n, double grad_scale, double max_norm, float* total_norm, float* clip_coef,
+                      void* workspace, size_t workspace_bytes, void* stream) {
+  if (!grad || n <= 0 || !total_norm || !clip_coef || !workspace || !(max_norm > 0.0)) {
+    set_last_error("pg_grad_norm_clip: bad argument");
+    return 1;
+  }
+  return grad_norm_clip(grad, n, grad_scale, max_norm, total_norm, clip_coef, workspace, workspace_bytes,
+                        reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pg_adamw_hf_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, double lr,
+                     double beta1, double beta2, double eps, double weight_decay, int64_t step, double grad_scale,
+                     const float* clip_coef, void* stream) {
+  if (!param || !grad || !exp_avg || !exp_avg_sq || n <= 0 || step < 1) {
+    set_last_error("pg_adamw_hf_step: bad argument");
+    return 1;
+  }
+  return adamw_hf_step(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, grad_scale,
+                       clip_coef, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // ---------------------------------------------------------------------------------------------- refiner

@@ -161,6 +161,40 @@ def clip_loss_grad(image_embeds: torch.Tensor, text_embeds: torch.Tensor, logit_
     return out
 
 
+def grad_norm_clip(grad: torch.Tensor, max_norm: float, grad_scale: float = 1.0,
+                   workspace: torch.Tensor | None = None):
+    """`torch.nn.utils.clip_grad_norm_` over one flat fp32 CUDA gradient read as grad * grad_scale, without modifying it:
+    -> (total_norm, clip_coef), two f32 CUDA scalars (clip_coef = min(max_norm / (total_norm + 1e-6), 1)); no host sync.
+    Deterministic.  A non-finite norm passes through (inf -> clip_coef 0, NaN -> NaN), as torch does."""
+    _need_cuda(grad, workspace)
+    if grad.dtype != torch.float32:
+        raise PigeonB200Error("grad_norm_clip needs an fp32 gradient")
+    lib = load()
+    n = grad.numel()
+    need = int(lib.pg_grad_norm_clip_workspace_bytes(n))
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=grad.device)
+    out = torch.empty(2, dtype=torch.float32, device=grad.device)
+    check(lib.pg_grad_norm_clip(ptr(grad), n, float(grad_scale), float(max_norm), ptr(out[0]), ptr(out[1]), ptr(workspace),
+                                workspace.numel(), current_stream_ptr()), "pg_grad_norm_clip")
+    return out[0], out[1]
+
+
+def adamw_hf_step(param: torch.Tensor, grad: torch.Tensor, exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, step: int,
+                  lr: float, betas=(0.9, 0.999), eps: float = 1e-6, weight_decay: float = 0.0, grad_scale: float = 1.0,
+                  clip_coef: torch.Tensor | None = None) -> None:
+    """transformers.optimization.AdamW.step (4.23.1, correct_bias=True) in place on one contiguous fp32 CUDA tensor;
+    `clip_coef` is an f32 CUDA scalar (None = 1), `step` counts from 1."""
+    _need_cuda(param, grad, exp_avg, exp_avg_sq, clip_coef)
+    if any(t.dtype != torch.float32 for t in (param, grad, exp_avg, exp_avg_sq)):
+        raise PigeonB200Error("adamw_hf_step needs fp32 parameter, gradient and state")
+    if not (param.numel() == grad.numel() == exp_avg.numel() == exp_avg_sq.numel()):
+        raise PigeonB200Error("adamw_hf_step: parameter, gradient and state sizes differ")
+    check(load().pg_adamw_hf_step(ptr(param), ptr(grad), ptr(exp_avg), ptr(exp_avg_sq), param.numel(), float(lr),
+                                  float(betas[0]), float(betas[1]), float(eps), float(weight_decay), int(step),
+                                  float(grad_scale), ptr(clip_coef), current_stream_ptr()), "pg_adamw_hf_step")
+
+
 def clip_project(x: torch.Tensor, w3: torch.Tensor, ln_weight: torch.Tensor | None = None,
                  ln_bias: torch.Tensor | None = None, eps: float = 1e-5) -> torch.Tensor:
     """x f32 [n, D] -> f32 [n, P] = LN(x) W^T (LN only when ln_weight / ln_bias are given), W packed by `head_pack_weight`

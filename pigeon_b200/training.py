@@ -8,6 +8,7 @@ evaluation and best-checkpoint saving per epoch — with `accelerate`/DDP replac
 from __future__ import annotations
 
 import logging
+import math
 from typing import Any, Callable, Dict, Iterable, Optional
 
 import torch
@@ -57,6 +58,143 @@ class AdamW:
                                           self.betas[0], self.betas[1], self.eps, self.weight_decay, st["step"], 1.0,
                                           current_stream_ptr()), "pg_adamw_step")
             _versions.bump(p)                                    # raw-pointer update: invalidate packed copies
+
+
+class AdamWHF(torch.optim.Optimizer):
+    """transformers.optimization.AdamW (transformers 4.23.1, `optim="adamw_hf"`, the HF Trainer's default optimizer, so the
+    one reference training/train_modes.py:30-64 pretrains with) as one fused CUDA kernel per parameter tensor
+    (pg_adamw_hf_step), fp32 state.  It differs from torch.optim.AdamW (`AdamW` above): eps is added to sqrt(v) before the
+    bias correction is folded into the step size, and the decoupled weight decay is applied after the update.
+
+    A torch Optimizer, so torch's LR schedulers drive `param_groups[i]["lr"]` and `state_dict()` has torch's layout
+    (per parameter: `step`, `exp_avg`, `exp_avg_sq`).  `step(clip_coef=, grad_scale=)` reads each gradient as
+    grad * grad_scale * clip_coef, with clip_coef an f32 CUDA scalar (from `ops.grad_norm_clip`), so no host sync."""
+
+    def __init__(self, params, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-6, weight_decay: float = 0.0,
+                 correct_bias: bool = True):
+        if lr < 0 or eps < 0 or weight_decay < 0 or not (0 <= betas[0] < 1) or not (0 <= betas[1] < 1):
+            raise ValueError("Invalid AdamWHF hyper-parameter")
+        if not correct_bias:
+            raise NotImplementedError("AdamWHF implements correct_bias=True (the HF Trainer's setting) only")
+        super().__init__(params, dict(lr=float(lr), betas=(float(betas[0]), float(betas[1])), eps=float(eps),
+                                      weight_decay=float(weight_decay), correct_bias=True))
+        self._lib = load()
+
+    @torch.no_grad()
+    def step(self, closure=None, clip_coef: Optional[torch.Tensor] = None, grad_scale: float = 1.0):
+        if closure is not None:
+            raise NotImplementedError("AdamWHF.step takes no closure")
+        stream = current_stream_ptr()
+        for group in self.param_groups:
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous():
+                    raise PigeonB200Error("AdamWHF: parameters and gradients must be contiguous fp32 CUDA tensors")
+                st = self.state[p]
+                if len(st) == 0:
+                    st["step"] = 0
+                    st["exp_avg"] = torch.zeros_like(p)
+                    st["exp_avg_sq"] = torch.zeros_like(p)
+                st["step"] += 1
+                check(self._lib.pg_adamw_hf_step(ptr(p), ptr(p.grad), ptr(st["exp_avg"]), ptr(st["exp_avg_sq"]), p.numel(),
+                                                 group["lr"], group["betas"][0], group["betas"][1], group["eps"],
+                                                 group["weight_decay"], int(st["step"]), float(grad_scale), ptr(clip_coef),
+                                                 stream), "pg_adamw_hf_step")
+                _versions.bump(p)                                # raw-pointer update: invalidate packed copies
+        return None
+
+
+# Modules of CLIPModel that are nn.LayerNorm in HF (our towers keep them in plain holder modules).
+_LAYERNORM_MODULES = ("layer_norm1", "layer_norm2", "final_layer_norm", "pre_layrnorm", "post_layernorm")
+_ATTN_ORDER = {"k_proj": 0, "v_proj": 1, "q_proj": 2, "out_proj": 3}
+
+
+def hf_named_parameters(model) -> list:
+    """`model.named_parameters()` in the order HF CLIPModel registers them (its attention holds k, v, q, out_proj in that
+    order), so that optimizer state lines up with an HF checkpoint's."""
+    named, out, i = list(model.named_parameters()), [], 0
+    while i < len(named):
+        if ".self_attn." not in named[i][0]:
+            out.append(named[i])
+            i += 1
+            continue
+        pre = named[i][0].split(".self_attn.")[0] + ".self_attn."
+        j = i
+        while j < len(named) and named[j][0].startswith(pre):
+            j += 1
+        out += sorted(named[i:j], key=lambda kv: _ATTN_ORDER[kv[0][len(pre):].split(".")[0]])   # stable: weight, bias
+        i = j
+    return out
+
+
+def decay_parameter_names(model) -> list:
+    """The HF Trainer rule (4.23.1 `create_optimizer`): `get_parameter_names(model, [nn.LayerNorm])` minus every name
+    containing "bias", restated by name.  `logit_scale`, the embeddings and `class_embedding` are decayed."""
+    return [n for n, _ in hf_named_parameters(model)
+            if n.rsplit(".", 1)[0].split(".")[-1] not in _LAYERNORM_MODULES and "bias" not in n]
+
+
+def optimizer_grouped_parameters(model, weight_decay: float) -> list:
+    """[decayed group, no-decay group] of the trainable parameters, each in HF parameter order (4.23.1 `create_optimizer`)."""
+    decay = set(decay_parameter_names(model))
+    named = [(n, p) for n, p in hf_named_parameters(model) if p.requires_grad]
+    return [{"params": [p for n, p in named if n in decay], "weight_decay": float(weight_decay)},
+            {"params": [p for n, p in named if n not in decay], "weight_decay": 0.0}]
+
+
+def linear_schedule_lambda(num_warmup_steps: int, num_training_steps: int) -> Callable[[int], float]:
+    """lr multiplier of `transformers.get_linear_schedule_with_warmup`: s / W during warm-up, then a linear decay to 0 at T."""
+    def lr_lambda(step: int) -> float:
+        if step < num_warmup_steps:
+            return float(step) / float(max(1, num_warmup_steps))
+        return max(0.0, float(num_training_steps - step) / float(max(1, num_training_steps - num_warmup_steps)))
+    return lr_lambda
+
+
+def schedule_lengths(num_examples: int, batch_size: int, grad_acc: int, world: int, epochs: float, max_steps: int = -1,
+                     warmup_steps: int = 0, warmup_ratio: float = 0.0):
+    """(batches per epoch per rank, updates per epoch, T, W, epochs to run) as the HF Trainer (4.23.1) derives them, with
+    a DistributedSampler (ceil(N / world) samples per rank) and drop-last batches."""
+    per_rank = -(-num_examples // world)
+    len_dataloader = per_rank // batch_size
+    updates_per_epoch = max(len_dataloader // grad_acc, 1)
+    if max_steps > 0:
+        total = int(max_steps)
+        n_epochs = max_steps // updates_per_epoch + int(max_steps % updates_per_epoch > 0)
+    else:
+        total = math.ceil(epochs * updates_per_epoch)
+        n_epochs = math.ceil(epochs)
+    warmup = int(warmup_steps) if warmup_steps > 0 else math.ceil(total * warmup_ratio)
+    return len_dataloader, updates_per_epoch, total, warmup, n_epochs
+
+
+def pretrain(model: Any, dataset, train_args=None, resume: bool = False, data_collator: Optional[Callable] = None):
+    """reference training/train_modes.py:30-64: contrastive pretraining of a CLIPModel with the HF Trainer's loop
+    (`pretrain.CLIPPretrainer`).  `model`: a `pigeon_b200.CLIPModel`, an HF `CLIPModel`, or a local directory / HF name.
+    `dataset['train']` / `dataset['val']` hold rows with pixel_values, input_ids (and attention_mask).  The validation
+    accuracy at batch size 16 is printed before and after training when the split has `.accuracy`.
+
+    Unlike the reference, which calls `trainer.train` only under `if resume:`, this always trains; `resume` resumes from
+    `train_args.resume_from_checkpoint` (None = start fresh, True = the latest checkpoint in output_dir)."""
+    from .clip_model import CLIPModel
+    from .pretrain import CLIPPretrainer
+    if train_args is None:
+        from .config import PRETAIN_ARGS as train_args
+    if isinstance(model, str):
+        model = CLIPModel.from_pretrained(model)
+    elif not isinstance(model, CLIPModel):
+        model = CLIPModel.from_hf(model)
+    model = model.to('cuda')
+    trainer = CLIPPretrainer(model, train_args, dataset['train'], eval_dataset=dataset['val'] if 'val' in dataset else None,
+                             data_collator=data_collator)
+    val = dataset['val'] if 'val' in dataset else None
+    if hasattr(val, 'accuracy'):
+        print('Before traing: Accuracy on batch size of 16 is', val.accuracy(model, batch_size=16))
+    trainer.train(resume_from_checkpoint=getattr(train_args, 'resume_from_checkpoint', None) if resume else None)
+    if hasattr(val, 'accuracy'):
+        print('After training: Accuracy on batch size of 16 is', val.accuracy(model, batch_size=16))
+    return model
 
 
 def _to_batch(data: Any) -> dict:

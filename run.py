@@ -6,9 +6,13 @@
     python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading]     # tower + head (run.py:165-169)
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
 
-`pretrain` (CLIP contrastive pre-training through the HF Trainer) is outside the path and raises NotImplementedError, like
-the reference does for its unsupported resume modes (run.py:166-173,189).  Datasets are HF `DatasetDict`s on disk, as in
-the reference (run.py:143-162); none are shipped with either repository.
+    python run.py pretrain openai/clip-vit-large-patch14-336 -l PRETRAIN_DATASET_DIR [--yfcc] [-r]          # (run.py:154-163)
+
+`pretrain` trains a CLIPModel contrastively with the HF Trainer loop of `pretrain.CLIPPretrainer` (PRETAIN_ARGS, or
+PRETAIN_ARGS_YFCC with --yfcc; -r passes its `resume_from_checkpoint` to the trainer, as the reference does).  Its dataset is a pre-processed
+`DatasetDict` with `train` and `val` splits whose rows hold pixel_values, input_ids and attention_mask; the caption synthesis
+of the reference's PretrainDataset is not part of this repository.  Datasets are HF `DatasetDict`s on disk, as in the
+reference (run.py:143-162); none are shipped with either repository.
 """
 import argparse
 import logging
@@ -62,26 +66,33 @@ def evaluate(model: str, dataset, yfcc: bool, landmarks: bool = False, base_mode
     return evaluate_model(full_model, dataset, metrics, None, refiner)
 
 
-def main():
-    p = argparse.ArgumentParser(description='PIGEON hot path on H100 (embed / evaluate)')
+def build_parser() -> argparse.ArgumentParser:
+    p = argparse.ArgumentParser(description='PIGEON hot path on H100 (pretrain / finetune / embed / evaluate)')
     p.add_argument('mode', choices=['pretrain', 'finetune', 'embed', 'evaluate'])
     p.add_argument('name', help='model / prediction-head path')
     p.add_argument('-l', '--load', default=None, help='comma-separated HF dataset directories')
     p.add_argument('-b', '--base', default=None, help='base (vision tower) checkpoint')
-    p.add_argument('-r', '--refine', action='store_true', default=True)
+    p.add_argument('--refine', action='store_true', default=True)
+    p.add_argument('-r', '--resume', action='store_true', help='pretrain: resume from train_args.resume_from_checkpoint (run.py:77-81)')
     p.add_argument('--yfcc', action='store_true')
     p.add_argument('--landmarks', action='store_true')
     p.add_argument('--heading', action='store_true')
     p.add_argument('-m', '--multitask', action='store_true')
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
-    args = p.parse_args()
-    if args.mode == 'pretrain':
-        raise NotImplementedError('"pretrain" (CLIP contrastive pre-training) is outside the H100 hot path')
+    return p
+
+
+def main(argv=None):
+    args = build_parser().parse_args(argv)
     if args.load is None:
         raise NotImplementedError('A dataset must be given with -l (the reference regenerates it from un-shipped raw data).')
     from datasets import DatasetDict
     dataset = DatasetDict.load_from_disk(args.load.split(',')[0])
-    if args.mode == 'finetune':
+    if args.mode == 'pretrain':
+        from pigeon_b200.training import pretrain
+        pretrain(args.name, dataset.with_format('torch'), cfg.PRETAIN_ARGS_YFCC if args.yfcc else cfg.PRETAIN_ARGS,
+                 resume=args.resume)
+    elif args.mode == 'finetune':
         from pigeon_b200.training import finetune_model, finetune_on_embeddings
         ds = dataset.with_format('torch')
         if args.embeddings:
