@@ -236,36 +236,39 @@ ln_backward_kernel(const float* __restrict__ dy, const float* __restrict__ x, co
 }
 
 // ------------------------------------------------------------------------------------------------ attention delta
-// Warp per row; float4 slot i of lane l covers columns 128 i + 4 l ..: head = 2 i + (l >> 4).
-template <int NV4>
+// Half-warp per (row, head) unit: lane l covers the head's columns 4 (l & 15) .. + 3, and a warp takes units 2 w and 2 w + 1
+// (for even head counts, two heads of one row).  Every unit's products and shuffle order do not depend on the head count.
 __global__ void __launch_bounds__(256)
 attention_delta_kernel(const float* __restrict__ d_out, const __half* __restrict__ out, float* __restrict__ delta,
-                       __nv_bfloat16* __restrict__ do_bf16, long rows, int seq) {
-  constexpr int hidden = NV4 * 128, heads = hidden / 64;
+                       __nv_bfloat16* __restrict__ do_bf16, long units, int seq, int heads) {
   const int lane = threadIdx.x & 31;
   const long warps = ((long)gridDim.x * blockDim.x) >> 5;
-  for (long row = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
+  for (long pair = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; 2 * pair < units; pair += warps) {
+    const long unit = 2 * pair + (lane >> 4);   // the loop bound is warp-uniform, so the full-warp shuffles below are legal
+    const bool ok = unit < units;
+    const long row = unit / heads;
+    const int head = (int)(unit - row * heads);
     const long view = row / seq;
     const int t = (int)(row - view * seq);
-    const float4* dr = reinterpret_cast<const float4*>(d_out + row * hidden);
-    const uint2* orow = reinterpret_cast<const uint2*>(out + row * hidden);
-    uint2* br = reinterpret_cast<uint2*>(do_bf16 + row * hidden);
-#pragma unroll
-    for (int i = 0; i < NV4; ++i) {
-      const float4 d = dr[lane + 32 * i];
-      const uint2 o = orow[lane + 32 * i];
-      const float2 o01 = __half22float2(*reinterpret_cast<const __half2*>(&o.x));
-      const float2 o23 = __half22float2(*reinterpret_cast<const __half2*>(&o.y));
-      float p = (d.x * o01.x + d.y * o01.y) + (d.z * o23.x + d.w * o23.y);
-#pragma unroll
-      for (int s = 8; s > 0; s >>= 1) p += __shfl_xor_sync(0xffffffffu, p, s);   // within each half-warp
-      if ((lane & 15) == 0) delta[(view * heads + 2 * i + (lane >> 4)) * seq + t] = p;
-      __nv_bfloat162 a = __floats2bfloat162_rn(d.x, d.y), b = __floats2bfloat162_rn(d.z, d.w);
-      uint2 pk;
-      pk.x = *reinterpret_cast<uint32_t*>(&a);
-      pk.y = *reinterpret_cast<uint32_t*>(&b);
-      br[lane + 32 * i] = pk;
+    const size_t col = (size_t)row * heads * 64 + head * 64 + 4 * (lane & 15);
+    float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+    uint2 o = make_uint2(0u, 0u);
+    if (ok) {
+      d = *reinterpret_cast<const float4*>(d_out + col);
+      o = *reinterpret_cast<const uint2*>(out + col);
     }
+    const float2 o01 = __half22float2(*reinterpret_cast<const __half2*>(&o.x));
+    const float2 o23 = __half22float2(*reinterpret_cast<const __half2*>(&o.y));
+    float p = (d.x * o01.x + d.y * o01.y) + (d.z * o23.x + d.w * o23.y);
+#pragma unroll
+    for (int s = 8; s > 0; s >>= 1) p += __shfl_xor_sync(0xffffffffu, p, s);   // within each half-warp
+    if (!ok) continue;
+    if ((lane & 15) == 0) delta[(view * heads + head) * seq + t] = p;
+    __nv_bfloat162 a = __floats2bfloat162_rn(d.x, d.y), b = __floats2bfloat162_rn(d.z, d.w);
+    uint2 pk;
+    pk.x = *reinterpret_cast<uint32_t*>(&a);
+    pk.y = *reinterpret_cast<uint32_t*>(&b);
+    *reinterpret_cast<uint2*>(do_bf16 + col) = pk;
   }
 }
 
@@ -389,16 +392,15 @@ int layernorm_backward(const float* dy, const float* x, const float* gamma, floa
 
 int attention_delta(const float* d_out, const void* out_f16, float* delta, void* do_bf16, int n_views, int seq, int heads,
                     int num_sms, cudaStream_t stream) {
-  const int hidden = heads * 64;
-  const long rows = (long)n_views * seq;
-  if (rows <= 0) return 0;
-  long blocks = (rows + 7) / 8;
+  if (heads <= 0) { set_last_error("attention_delta: heads %d < 1", heads); return 1; }
+  const long units = (long)n_views * seq * heads;
+  if (units <= 0) return 0;
+  long blocks = (units + 15) / 16;   // 8 warps per block, two units per warp
   const long cap = (long)(num_sms > 0 ? num_sms : 132) * 8;
   if (blocks > cap) blocks = cap;
   ProfScope prof("train_attention_delta", stream);
-  PG_DISPATCH_NV4(hidden, (attention_delta_kernel<NV4><<<(int)blocks, 256, 0, stream>>>(
-                              d_out, reinterpret_cast<const __half*>(out_f16), delta,
-                              reinterpret_cast<__nv_bfloat16*>(do_bf16), rows, seq)));
+  attention_delta_kernel<<<(int)blocks, 256, 0, stream>>>(d_out, reinterpret_cast<const __half*>(out_f16), delta,
+                                                          reinterpret_cast<__nv_bfloat16*>(do_bf16), units, seq, heads);
   return check_launch("attention_delta");
 }
 
