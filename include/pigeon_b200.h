@@ -536,6 +536,28 @@ int pg_dgelu_bf16(const float* dh, const void* u, void* du, int64_t n, void* str
 int pg_transpose_to_bf16(const void* src, int32_t src_type, int64_t lds, void* out, int64_t ldo, int64_t rows, int32_t cols,
                          void* stream);
 
+/* ---------------------------------------------------------------------------------------------------
+ * Prototype clustering: the per-geocell OPTICS-xi of reference dataset_creation/prototype/prototype.py:121-145
+ * (`ProtoDataset._compute_distances`, `_compute_clusters`), i.e. for every cell
+ *   sklearn.cluster.OPTICS(min_samples=m, xi=xi, metric='precomputed').fit_predict(D)
+ * with D the fp64 haversine matrix of the cell in km (exact zeros read as 1e-5), restating scikit-learn's
+ * compute_optics_graph (max_eps = inf), cluster_optics_xi (min_cluster_size = m, predecessor_correction = True),
+ * _xi_cluster and _extract_xi_labels.  D is recomputed on the fly, never stored.
+ * ------------------------------------------------------------------------------------------------- */
+/* Bytes of workspace pg_optics_xi needs for N points in num_cells cells (about 90 bytes per point). */
+size_t pg_optics_workspace_bytes(int64_t N, int32_t num_cells);
+/* lnglat_deg f64 [N, 2] (lng, lat in degrees, finite) holds the points grouped by cell: cell c is rows
+ * [cell_off[c], cell_off[c+1]) (cell_off i64 [num_cells + 1], cell_off[0] = 0, cell_off[num_cells] = N; empty cells allowed).
+ * max_cell is the host-known largest cell size (it sizes shared memory only).  Writes labels_out i32 [N], the cell-local
+ * OPTICS-xi label of every point (-1 = noise); a cell of fewer than min_samples points gets label 0 everywhere
+ * (prototype.py:144-145).  The optional outputs (NULL = not written) are OPTICS' ordering_ (cell-local indices, at the
+ * cell's rows), core_distances_, reachability_ and predecessor_ (cell-local, -1 = none) per point; for a cell below
+ * min_samples they hold -1 / NaN / NaN / -1.  Deterministic; no host synchronisation.
+ * Fails for min_samples < 2, xi outside (0, 1) or a workspace that is too small. */
+int pg_optics_xi(const double* lnglat_deg, int64_t N, const int64_t* cell_off, int32_t num_cells, int64_t max_cell,
+                 int32_t min_samples, double xi, void* workspace, size_t workspace_bytes, int32_t* labels_out,
+                 int64_t* ordering_out, double* reach_out, double* core_out, int64_t* pred_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -39,6 +39,7 @@ SOURCES = [
     "clip_capi.cu",
     "clip_train.cu",
     "pretrain.cu",
+    "optics.cu",
 ]
 
 NVCC_FLAGS = [

@@ -164,6 +164,9 @@ SIGNATURES = {
     "pg_grad_norm_clip": (c_int32, [c_void_p, c_int64, c_double, c_double, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "pg_adamw_hf_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_double, c_double, c_double, c_double,
                                    c_double, c_int64, c_double, c_void_p, c_void_p]),
+    "pg_optics_workspace_bytes": (c_size_t, [c_int64, c_int32]),
+    "pg_optics_xi": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_int64, c_int32, c_double, c_void_p, c_size_t,
+                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pg_refiner_workspace_bytes": (c_size_t, [c_int64, c_int32, c_int32, c_int32]),
     "pg_refiner_forward": (c_int32, [C.POINTER(RefinerBank), c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p,
                                      c_int32, c_int32, c_float, c_double, c_void_p, c_size_t, c_void_p, c_void_p,
