@@ -558,6 +558,60 @@ int pg_optics_xi(const double* lnglat_deg, int64_t N, const int64_t* cell_off, i
                  int32_t min_samples, double xi, void* workspace, size_t workspace_bytes, int32_t* labels_out,
                  int64_t* ordering_out, double* reach_out, double* core_out, int64_t* pred_out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * GeoGuessr evaluation metrics (csrc/geo_metrics.cu): reference evaluation/metrics.py compute_geoguessr_metrics.
+ *
+ * Countries are Polygon / MultiPolygon geometries as CSR arrays, in feature order: verts f64 [num_verts, 2] (lng, lat,
+ * finite); ring r is verts[ring_off[r] .. ring_off[r+1]) and is closed (last == first, at least 4 positions); part p
+ * (one polygon: its shell, then its holes) is rings [part_ring_off[p], part_ring_off[p+1]); geometry q is parts
+ * [geom_part_off[q], geom_part_off[q+1]).  Every offset array is i64, starts at 0 and ends at the next level's count.
+ * The index (pg_country_index_bytes) holds bounding boxes and per-part latitude bands; `entries` (i32 [num_entries])
+ * lists each band's edges.  Build: pg_country_index_build writes the entry count to *num_entries_out (device i64);
+ * the caller allocates the entries and calls pg_country_index_fill.  Both are deterministic.
+ * ------------------------------------------------------------------------------------------------------------- */
+typedef struct {
+  const double* verts;
+  const int64_t* ring_off;
+  const int64_t* part_ring_off;
+  const int64_t* geom_part_off;
+  int64_t num_verts, num_rings, num_parts, num_geoms;
+  void* index;
+  size_t index_bytes;
+  int32_t* entries;
+  int64_t num_entries;
+} PgCountries;
+
+#define PG_COUNTRY_NEAREST 1 /* flags: the label is covered by no geometry; its country is the nearest one */
+
+size_t pg_country_index_bytes(int64_t num_verts, int64_t num_parts, int64_t num_geoms);
+int pg_country_index_build(const PgCountries* countries, int64_t* num_entries_out, void* stream);
+int pg_country_index_fill(const PgCountries* countries, void* stream);
+/* Per sample n (label_lnglat, pred_lnglat f64 [N, 2]): country_out i32 = the lowest-index geometry that covers the label
+ * (boundary included), else the nearest geometry by GEOS Distance::pointToSegment in degrees (lowest index on exact
+ * ties) with PG_COUNTRY_NEAREST in flags_out u8; pred_inside_out u8 (optional) = that geometry contains the prediction
+ * (interior only).  Exact orientation predicates, GEOS semantics (DESIGN.md §1).  No host synchronisation. */
+int pg_country_locate(const PgCountries* countries, const double* label_lnglat, const double* pred_lnglat, int64_t N,
+                      int32_t* country_out, uint8_t* flags_out, uint8_t* pred_inside_out, void* stream);
+
+/* results_out f64 [PG_GEO_NUM_RESULTS] of pg_geo_metrics */
+#define PG_GEO_MEAN_KM 0
+#define PG_GEO_MEDIAN_KM 1
+#define PG_GEO_UNDER_KM 2 /* 10 shares: distance < 1, 5, 10, 25, 50, 100, 200, 750, 1000, 2500 km */
+#define PG_GEO_COUNTRY 12
+#define PG_GEO_SCORE 13
+#define PG_GEO_TOP1 14
+#define PG_GEO_TOPK 15
+#define PG_GEO_NUM_RESULTS 16
+size_t pg_geo_metrics_workspace_bytes(int64_t N);
+/* One pass over N >= 1 samples: pred_lnglat [N, 2] (f32 when pred_is_f32, else f64), label_lnglat f64 [N, 2],
+ * cell_pred / cell_label i64 [N], topk i64 [N, k], pred_inside u8 [N] (pg_country_locate).  Writes dist_out f64 [N]
+ * (haversine_np km, numpy 2 dtype rules) and results_out: mean and median (np.median) km, the Under_*_km shares, country
+ * accuracy, mean GeoGuessr score, top-1 and top-k geocell accuracy.  Fixed-order reductions; no host synchronisation. */
+int pg_geo_metrics(const void* pred_lnglat, int32_t pred_is_f32, const double* label_lnglat, int64_t N,
+                   const int64_t* cell_pred, const int64_t* cell_label, const int64_t* topk, int32_t k,
+                   const uint8_t* pred_inside, void* workspace, size_t workspace_bytes, double* dist_out,
+                   double* results_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

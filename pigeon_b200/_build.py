@@ -40,6 +40,7 @@ SOURCES = [
     "clip_train.cu",
     "pretrain.cu",
     "optics.cu",
+    "geo_metrics.cu",
 ]
 
 NVCC_FLAGS = [

@@ -83,6 +83,12 @@ class RefinerBank(C.Structure):
                 ("member_idx", c_void_p), ("data_emb", c_void_p), ("data_lnglat", c_void_p), ("proto_sqnorm", c_void_p), ("num_protos", c_int64), ("live_cells", c_int32)]
 
 
+class PgCountries(C.Structure):
+    _fields_ = [("verts", c_void_p), ("ring_off", c_void_p), ("part_ring_off", c_void_p), ("geom_part_off", c_void_p),
+                ("num_verts", c_int64), ("num_rings", c_int64), ("num_parts", c_int64), ("num_geoms", c_int64),
+                ("index", c_void_p), ("index_bytes", c_size_t), ("entries", c_void_p), ("num_entries", c_int64)]
+
+
 class GemmProblem(C.Structure):
     _fields_ = [("M", c_int32), ("N", c_int32), ("K", c_int32), ("a", c_void_p), ("lda", c_int32), ("w", c_void_p),
                 ("ldw", c_int32), ("out", c_void_p), ("ldo", c_int32), ("bias", c_void_p), ("epilogue", c_int32),
@@ -167,6 +173,14 @@ SIGNATURES = {
     "pg_optics_workspace_bytes": (c_size_t, [c_int64, c_int32]),
     "pg_optics_xi": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_int64, c_int32, c_double, c_void_p, c_size_t,
                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pg_country_index_bytes": (c_size_t, [c_int64, c_int64, c_int64]),
+    "pg_country_index_build": (c_int32, [C.POINTER(PgCountries), c_void_p, c_void_p]),
+    "pg_country_index_fill": (c_int32, [C.POINTER(PgCountries), c_void_p]),
+    "pg_country_locate": (c_int32, [C.POINTER(PgCountries), c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]),
+    "pg_geo_metrics_workspace_bytes": (c_size_t, [c_int64]),
+    "pg_geo_metrics": (c_int32, [c_void_p, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_void_p,
+                                 c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
     "pg_refiner_workspace_bytes": (c_size_t, [c_int64, c_int32, c_int32, c_int32]),
     "pg_refiner_forward": (c_int32, [C.POINTER(RefinerBank), c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p,
                                      c_int32, c_int32, c_float, c_double, c_void_p, c_size_t, c_void_p, c_void_p,

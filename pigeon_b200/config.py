@@ -10,6 +10,16 @@ CLIP_EMBED_DIM = 1024
 GEOCELL_PATH = 'data/geocells_2203.csv'       # PIGEON
 GEOCELL_PATH_YFCC = 'data/geocells_yfcc.csv'  # PIGEOTTO
 
+# Country borders for Country_accuracy (a GeoJSON FeatureCollection supplied by the user)   (config.py:26)
+COUNTRY_PATH = 'data/geocells/countries.geojson'
+
+# Multi-task regression scalers (joblib StandardScaler)             (config.py:39-40)
+SCALER_PATH = 'saved_models/scaler/regression.scaler'
+SCALER_PATH_YFCC = 'saved_models/scaler/regression_yfcc.scaler'
+
+# GeoGuessr score decay, in km                                         (config.py:52)
+DECAY_CONSTANT = 1492.7
+
 # Haversine smoothing constant                                         (config.py:54-56)
 LABEL_SMOOTHING_CONSTANT = 65
 

@@ -6,8 +6,8 @@
 //
 // Four kernels per call, all on the caller's stream:
 //   prep      per point: deg2rad and cos(lat) (numpy forms these per point too);
-//   core      one CTA per point: the m-th smallest entry of its row by a 6-pass radix select (11-bit digits) on the
-//             uint64 bit pattern of the distance (all distances are positive, so bit order is value order);
+//   core      one CTA per point: the m-th smallest entry of its row by radix_select.cuh's exact 6-pass radix select
+//             on the uint64 bit pattern of the distance (all distances are positive, so bit order is value order);
 //   ordering  one CTA per cell, largest cells first: n steps of "mark p processed, update every unprocessed j, arg-min";
 //             the update and the next arg-min are one pass plus one block reduction;
 //   xi        one thread per cell: sklearn's _xi_cluster + _extract_xi_labels on the reachability plot.
@@ -17,6 +17,7 @@
 #include <stdint.h>
 
 #include "../../include/pigeon_b200.h"
+#include "radix_select.cuh"
 #include "tma_host.h"
 
 namespace pg {
@@ -112,64 +113,18 @@ __global__ void cell_order_kernel(const int64_t* __restrict__ cell_off, int32_t 
 
 // core[i] = around(m-th smallest of row i of D, 15): NearestNeighbors.kneighbors(X, m)[0][:, -1] of a precomputed
 // matrix, the diagonal included (sklearn/cluster/_optics.py _compute_core_distances_, compute_optics_graph).
-// Radix select on the bit pattern, most significant digit first: bits 53-63, 42-52, 31-41, 20-30, 9-19, 0-8.  Each pass
-// recomputes the row (no per-row storage, any m); when the selected digit holds one candidate, one more pass fetches it.
+// Exact radix select (radix_select.cuh); each pass recomputes the row, so there is no per-row storage and any m works.
 __global__ void __launch_bounds__(CORE_THREADS) core_kernel(const int64_t* __restrict__ cell_off, int32_t C, int32_t m,
                                                             Ws w) {
-  __shared__ uint32_t hist[2048];
-  __shared__ uint64_t s_prefix;
-  __shared__ uint32_t s_k, s_cnt;
   const int64_t i = blockIdx.x;
   const int64_t c = find_cell(cell_off, C, i);
   const int64_t b = cell_off[c], n = cell_off[c + 1] - b;
   if (n < m) return;
   const double li = w.lng[i], ai = w.lat[i], ci = w.coslat[i];
-  if (threadIdx.x == 0) { s_prefix = 0; s_k = uint32_t(m); }
-  int hi_shift = 64;
-  for (int pass = 0; pass < 6; ++pass) {
-    const int width = pass < 5 ? 11 : 9, shift = hi_shift - width;
-    const uint32_t bins = 1u << width;
-    for (uint32_t t = threadIdx.x; t < bins; t += CORE_THREADS) hist[t] = 0;
-    __syncthreads();
-    const uint64_t prefix = s_prefix;
-    for (int64_t j = threadIdx.x; j < n; j += CORE_THREADS) {
-      const uint64_t v = __double_as_longlong(haversine_km(li, ai, ci, w.lng[b + j], w.lat[b + j], w.coslat[b + j]));
-      if (hi_shift == 64 || (v >> hi_shift) == (prefix >> hi_shift)) atomicAdd(&hist[(v >> shift) & (bins - 1)], 1u);
-    }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      const uint32_t lane = threadIdx.x, per = bins / 32, k = s_k;
-      uint32_t sum = 0;
-      for (uint32_t t = 0; t < per; ++t) sum += hist[lane * per + t];
-      uint32_t incl = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= uint32_t(o)) incl += y;
-      }
-      const uint32_t excl = incl - sum;
-      if (excl < k && k <= incl) {
-        uint32_t acc = excl, d = lane * per;
-        while (acc + hist[d] < k) acc += hist[d++];
-        s_prefix = prefix | (uint64_t(d) << shift);
-        s_k = k - acc;
-        s_cnt = hist[d];
-      }
-    }
-    __syncthreads();
-    hi_shift = shift;
-    if (s_cnt == 1 && shift > 0) {  // one candidate left: fetch its remaining bits
-      const uint64_t pre = s_prefix;
-      __syncthreads();  // every thread holds the prefix before the one match overwrites it
-      for (int64_t j = threadIdx.x; j < n; j += CORE_THREADS) {
-        const uint64_t v = __double_as_longlong(haversine_km(li, ai, ci, w.lng[b + j], w.lat[b + j], w.coslat[b + j]));
-        if ((v >> shift) == (pre >> shift)) s_prefix = v;
-      }
-      __syncthreads();
-      break;
-    }
-  }
-  if (threadIdx.x == 0) w.core[i] = around15(__longlong_as_double(s_prefix));
+  const uint64_t kth = radix_select_kth<CORE_THREADS>(n, uint32_t(m), [&](int64_t j) {
+    return uint64_t(__double_as_longlong(haversine_km(li, ai, ci, w.lng[b + j], w.lat[b + j], w.coslat[b + j])));
+  });
+  if (threadIdx.x == 0) w.core[i] = around15(__longlong_as_double(kth));
 }
 
 // compute_optics_graph's main loop (max_eps = inf) for one cell: at each step the unprocessed point of least

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Entry points of the hot path with the reference's CLI (run.py:21-93): `embed`, `evaluate` and `finetune`.
 
-    python run.py evaluate HEAD.model -l DATASET_DIR [-b BASE.model] [--yfcc]
+    python run.py evaluate HEAD.model -l DATASET_DIR [-b BASE.model] [--yfcc] [--metrics]
     python run.py embed CLIP.model -l DATASET_DIR
     python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading]     # tower + head (run.py:165-169)
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
@@ -13,6 +13,10 @@ PRETAIN_ARGS_YFCC with --yfcc; -r passes its `resume_from_checkpoint` to the tra
 `DatasetDict` with `train` and `val` splits whose rows hold pixel_values, input_ids and attention_mask; the caption synthesis
 of the reference's PretrainDataset is not part of this repository.  Datasets are HF `DatasetDict`s on disk, as in the
 reference (run.py:143-162); none are shipped with either repository.
+
+`--metrics` (evaluate, finetune) evaluates with `metrics.compute_geoguessr_metrics`, as the reference's evaluate.py and
+train_modes.py do: the full GeoGuessr table, with Country_accuracy against config.COUNTRY_PATH.  Without it only
+Geocell_accuracy is computed.
 """
 import argparse
 import logging
@@ -79,7 +83,17 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument('--heading', action='store_true')
     p.add_argument('-m', '--multitask', action='store_true')
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
+    p.add_argument('--metrics', action='store_true',
+                   help='evaluate / finetune: report compute_geoguessr_metrics (needs config.COUNTRY_PATH)')
     return p
+
+
+def metrics_fn(args):
+    """The `metrics` callable evaluate_model gets: compute_geoguessr_metrics with --metrics, else None."""
+    if not args.metrics:
+        return None
+    from pigeon_b200.metrics import compute_geoguessr_metrics
+    return compute_geoguessr_metrics
 
 
 def main(argv=None):
@@ -96,16 +110,18 @@ def main(argv=None):
         from pigeon_b200.training import finetune_model, finetune_on_embeddings
         ds = dataset.with_format('torch')
         if args.embeddings:
-            finetune_on_embeddings(ds, multi_task=args.multitask, heading=args.heading, yfcc=args.yfcc)   # run.py:175
+            finetune_on_embeddings(ds, multi_task=args.multitask, heading=args.heading, yfcc=args.yfcc,
+                                   metrics=metrics_fn(args))                                                 # run.py:175
         else:
-            finetune_model(args.name, ds, multi_task=args.multitask, heading=args.heading, yfcc=args.yfcc)  # run.py:169
+            finetune_model(args.name, ds, multi_task=args.multitask, heading=args.heading, yfcc=args.yfcc,
+                           metrics=metrics_fn(args))                                                          # run.py:169
     elif args.mode == 'embed':
         model = CLIPEmbedding(args.name, load_checkpoint=True, panorama=not args.yfcc)    # run.py:126-129
         embed_images(model, dataset)
     else:
         split = dataset['test'] if 'test' in dataset else dataset[list(dataset.keys())[-1]]
         print(evaluate(args.name, split.with_format('torch'), args.yfcc, args.landmarks, base_model=args.base,
-                       heading=args.heading, refine=args.refine))
+                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args)))
 
 
 if __name__ == '__main__':
