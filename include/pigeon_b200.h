@@ -499,7 +499,8 @@ int pg_layernorm_f16(const float* x, void* y, const float* gamma, const float* b
 int pg_attention_f16(const void* qkv, void* out, int32_t n_views, int32_t seq, int32_t heads, void* stream);
 /* The text tower's attention (HF CLIPTextTransformer: causal mask + expanded attention_mask, 4.23.1): key j is admissible
  * for query i only if (causal == 0 or j <= i) and (mask == NULL or mask[view, j] != 0); mask i64 [n_views, seq],
- * mask[:, 0] must be non-zero.  mask NULL and causal 0 is pg_attention_f16, bit for bit. */
+ * mask[:, 0] must be non-zero.  mask NULL and causal 0 is pg_attention_f16, bit for bit.  The models pass a 0/1 mask
+ * (HF excludes every key whose attention_mask is not exactly 1; CLIPTextTower and the text trainer map it so on the host). */
 int pg_attention_f16_masked(const void* qkv, void* out, const int64_t* mask, int32_t causal, int32_t n_views, int32_t seq,
                             int32_t heads, void* stream);
 /* The same op with the optional lse2 side output (may be NULL).  `variant` (0..3) and `poly` selected among several forward

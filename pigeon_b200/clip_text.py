@@ -52,6 +52,12 @@ def _strip_prefix(sd: Dict[str, Tensor]) -> Dict[str, Tensor]:
     return out
 
 
+def admissible_keys(attention_mask: Tensor) -> Tensor:
+    """attention_mask [n, S] of any dtype -> the kernels' 0/1 int64 mask.  HF 4.23.1's `_expand_mask` adds finfo.min
+    wherever `1 - mask` is nonzero, so a key is attended only where its mask is exactly 1 (2, -1 or 1.5 exclude it)."""
+    return (attention_mask == 1).to(torch.int64).contiguous()
+
+
 def check_sequence_length(S: int, max_positions: int) -> None:
     """HF CLIPTextEmbeddings rejects sequences longer than the position table (the message of transformers 4.23.1+)."""
     if S > max_positions:
@@ -162,7 +168,7 @@ class TextEngine:
         if attention_mask is not None:
             if tuple(attention_mask.shape) != (n, S):
                 raise ValueError(f"attention_mask {tuple(attention_mask.shape)} does not match input_ids {(n, S)}")
-            mask = attention_mask.to(device=self.device, dtype=torch.int64).contiguous()
+            mask = admissible_keys(attention_mask.to(self.device))
         pooled = torch.empty((n, d.hidden), dtype=torch.float32, device=self.device)
         hidden = torch.empty((n, S, d.hidden), dtype=torch.float32, device=self.device) if return_hidden else None
         if n == 0:

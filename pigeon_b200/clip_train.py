@@ -14,6 +14,7 @@ import torch
 
 from . import _lib
 from ._lib import PigeonB200Error, check, current_stream_ptr, load, ptr
+from .clip_text import admissible_keys
 from .vit_train import (LAYER_GRADS, _aligned_empty, _align, layer_grad_shapes, put_grad, put_layer_grads,
                         transpose_layers)
 
@@ -89,7 +90,7 @@ class TextTrainer:
         d = self.dims
         n, S = input_ids.shape
         ids = input_ids.to(dtype=torch.int64).contiguous()
-        mask = None if attention_mask is None else attention_mask.to(dtype=torch.int64).contiguous()
+        mask = None if attention_mask is None else admissible_keys(attention_mask)
         self._build_saved(n, S)
         self._inputs = (ids, mask)
         eng = self.tower.engine()

@@ -143,3 +143,15 @@ def test_clip_argument_errors_before_any_kernel():
         m(input_ids=torch.ones(1, 9, dtype=torch.int64), pixel_values=torch.zeros(1, 3, 28, 28))
     with pytest.raises(ValueError):
         m(input_ids=torch.ones(2, 4, dtype=torch.int64), pixel_values=torch.zeros(1, 3, 28, 28), return_loss=True)
+
+
+def test_attention_mask_admits_only_ones():
+    """HF's `_expand_mask` excludes every key whose mask is not exactly 1; the kernels get that as a 0/1 int64 mask."""
+    from pigeon_b200.clip_text import admissible_keys
+    m = torch.tensor([[1, 0, 2, -1, 1.5, 0.5, 1], [1, 1, 1, 1, 1, 1, 0]], dtype=torch.float64)
+    want = torch.tensor([[1, 0, 0, 0, 0, 0, 1], [1, 1, 1, 1, 1, 1, 0]])
+    for t in (m, m.float(), m.half(), m.to(torch.int64)):
+        got = admissible_keys(t)
+        assert got.dtype == torch.int64 and got.is_contiguous()
+        assert torch.equal(got, want if t.is_floating_point() else (m.to(torch.int64) == 1).to(torch.int64))
+    assert torch.equal(admissible_keys(torch.tensor([[True, False]])), torch.tensor([[1, 0]]))

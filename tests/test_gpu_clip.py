@@ -108,17 +108,35 @@ def test_vit_forward_cls(cuda, fold):
 
 
 # ------------------------------------------------------------------------------------------------ text tower
-def _text_vs_oracle(cuda, td, lengths, seed, std):
-    import clip_oracle
+def _text_tower(cuda, td, seed, std):
     from pigeon_b200 import CLIPTextTower, synthetic
     from pigeon_b200.vit_engine import VitDims
     vd = VitDims(image_size=28, patch_size=14, hidden=256, heads=4, intermediate=512, layers=1)
     sd = synthetic.random_clip_state_dict(td, vd, seed=seed, std=std)
-    ids, mask = _captions(lengths, td.vocab, seed + 1)
     tower = CLIPTextTower(td)
     tower.load_state_dict({k: v for k, v in sd.items() if k.startswith("text_model.")})
     tower = tower.to(cuda)
     tower.max_texts_per_pass = 3
+    return tower, sd
+
+
+def _odd_mask(mask):
+    """(float mask with 2, -1 and 1.5 in place of some of the ones after key 0, the same mask with those entries 0).  HF's
+    `_expand_mask` excludes every key whose mask is not exactly 1."""
+    odd = mask.double().clone()
+    values = [2.0, -1.0, 1.5]
+    for b in range(odd.shape[0]):
+        for i, j in enumerate(range(1 + b % 2, int(mask[b].sum()), 2)):
+            odd[b, j] = values[(b + i) % 3]
+    return odd, torch.where(odd == 1, odd, torch.zeros_like(odd))
+
+
+def _text_vs_oracle(cuda, td, lengths, seed, std, odd_mask=False):
+    import clip_oracle
+    tower, sd = _text_tower(cuda, td, seed, std)
+    ids, mask = _captions(lengths, td.vocab, seed + 1)
+    if odd_mask:
+        mask, _ = _odd_mask(mask)
     out = tower(input_ids=ids.to(cuda), attention_mask=mask.to(cuda))
     torch.cuda.synchronize()
     ref_h, ref_p = clip_oracle.text_forward(sd, ids, mask, heads=td.heads, layers=td.layers, eps=td.ln_eps)
@@ -136,6 +154,27 @@ def test_text_tower_tiny(cuda):
     e_h, e_p, e_t = _text_vs_oracle(cuda, td, [12, 5, 9, 1, 16, 2, 7], seed=3, std=0.05)
     print(f"text tower tiny rel-L2: last_hidden_state {e_h:.3e} pooled {e_p:.3e} text_embeds {e_t:.3e}")
     assert e_h < REL_TOL and e_p < REL_TOL and e_t < REL_TOL, (e_h, e_p, e_t)
+
+
+def test_text_tower_excludes_mask_values_other_than_one(cuda):
+    """attention_mask entries 2, -1 and 1.5 exclude their keys, as in HF: the tower matches the oracle, and both the tower
+    and the trainer's forward give the bits of the same mask with those entries 0."""
+    from pigeon_b200 import TextDims
+    from pigeon_b200.clip_train import TextTrainer
+    td = TextDims(vocab=1000, max_positions=16, hidden=256, heads=4, intermediate=512, layers=2)
+    e_h, e_p, e_t = _text_vs_oracle(cuda, td, [12, 5, 9, 1, 16, 2, 7], seed=3, std=0.05, odd_mask=True)
+    assert e_h < REL_TOL and e_p < REL_TOL and e_t < REL_TOL, (e_h, e_p, e_t)
+    tower, _ = _text_tower(cuda, td, seed=3, std=0.05)
+    ids, mask = _captions([12, 5, 9, 1, 16, 2, 7], td.vocab, 4)
+    odd, zeroed = _odd_mask(mask)
+    assert (odd != zeroed).any() and (odd[:, 0] == 1).all()
+    ids, odd, zeroed = ids.to(cuda), odd.to(cuda), zeroed.to(cuda)
+    a, b = tower(input_ids=ids, attention_mask=odd), tower(input_ids=ids, attention_mask=zeroed)
+    assert torch.equal(a.last_hidden_state, b.last_hidden_state) and torch.equal(a.pooler_output, b.pooler_output)
+    tt = TextTrainer(tower)
+    pa = tt.forward(ids, odd).clone()
+    pb = tt.forward(ids, zeroed)
+    assert torch.equal(pa, pb)
 
 
 def test_text_tower_large(cuda):
