@@ -197,6 +197,50 @@ int pg_preprocess_clip(const pg_image* images, int32_t n, int32_t size, const fl
                        void* workspace, size_t workspace_bytes, void* out, int32_t out_f16, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Baseline JPEG decoding (csrc/jpeg.cu): what `PIL.Image.open(f).convert('RGB')` does on the CPU before every
+ * CLIPProcessor call in reference dataset_creation/finetune/embed_dataset.py:17-22 (through the HF Image() column of
+ * finetune_dataset.py:86-90), dataset_creation/benchmark/benchmark_dataset.py:66-79 and pretrain_dataset.py:109-161.
+ * Byte-identical to Pillow over libjpeg-turbo with its defaults (ISLOW IDCT, fancy upsampling) for the files it
+ * decodes: sequential Huffman (SOF0 / SOF1), 8-bit, one scan, grayscale or YCbCr 4:4:4 / 4:2:2 / 4:2:0, with or
+ * without restart markers.  Everything else is refused with a status and a reason (DESIGN.md §1).
+ * ------------------------------------------------------------------------------------------------- */
+#define PG_JPEG_OK 0
+#define PG_JPEG_UNSUPPORTED 1       /* a valid file outside the decoded subset: progressive, 12-bit, CMYK, RGB, ... */
+#define PG_JPEG_BAD_HEADER 2        /* truncated or inconsistent marker segments, or not a JPEG */
+#define PG_JPEG_BAD_CODE 3          /* entropy data: a code missing from its table, or a run past coefficient 63 */
+#define PG_JPEG_OVERRUN 4           /* entropy data: a segment ends before its MCUs do */
+#define PG_JPEG_UNEXPECTED_MARKER 5 /* entropy data: a marker where data should be */
+#define PG_JPEG_BAD_RST 6           /* entropy data: wrong restart marker number or count */
+#define PG_JPEG_NO_EOI 7            /* entropy data: the file ends without EOI */
+
+typedef struct pg_jpeg_info {
+  int32_t status;                 /* PG_JPEG_* */
+  int32_t sof;                    /* frame marker (0xC0 .. 0xCF), 0 before one is seen */
+  int32_t precision, height, width, components;
+  int32_t component_id[3], h_samp[3], v_samp[3], quant_table[3], dc_table[3], ac_table[3];
+  int32_t restart_interval;       /* MCUs per restart interval, 0 without DRI */
+  int32_t num_segments;           /* entropy-coded segments: restart intervals, or 1 */
+  int32_t table_mask;             /* bit t: DQT t defined; bit 4 + t: DC DHT t; bit 8 + t: AC DHT t */
+  int64_t scan_offset, scan_bytes; /* entropy-coded data, from the end of the SOS segment to the marker after it */
+  uint16_t qt[4][64];             /* quantisation tables in zig-zag order, as stored */
+  uint8_t dc_bits[4][16], ac_bits[4][16];
+  uint8_t dc_vals[4][256], ac_vals[4][256];
+} pg_jpeg_info;
+
+/* Host-only marker walk of one file (data_host: `bytes` bytes).  Returns info_out->status; when it is not PG_JPEG_OK,
+ * pg_last_error() names the reason.  Validates the restart-marker sequence and the EOI. */
+int pg_jpeg_parse(const uint8_t* data_host, int64_t bytes, pg_jpeg_info* info_out);
+/* Workspace of pg_jpeg_decode for n parsed files packed into packed_bytes bytes.  0 on error. */
+size_t pg_jpeg_workspace_bytes(const pg_jpeg_info* infos_host, int32_t n, int64_t packed_bytes);
+/* Decodes the files whose info status is PG_JPEG_OK: file i is packed_host[offsets_host[i] .. offsets_host[i+1]) (one
+ * host-to-device copy of offsets_host[n] bytes; pinned memory makes it asynchronous), infos_host[i] its pg_jpeg_parse
+ * result, dst_host[i] a descriptor of its height x width x 3 uint8 RGB destination (written; the same descriptors feed
+ * pg_preprocess_clip).  status_out: device i32 [n], the parse status of a skipped file, else PG_JPEG_OK or the
+ * entropy-data error of that file (whose destination is then left unwritten).  Three launches for the whole batch. */
+int pg_jpeg_decode(const uint8_t* packed_host, const int64_t* offsets_host, const pg_jpeg_info* infos_host, int32_t n,
+                   const pg_image* dst_host, void* workspace, size_t workspace_bytes, int32_t* status_out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Fine-tune step, head-only part ("next" row N1 with a frozen or absent base model): what loss.backward() and
  * torch.optim.AdamW.step() do for cell_layer in reference training/train_eval_loop.py:187,215-221.
  * ------------------------------------------------------------------------------------------------- */

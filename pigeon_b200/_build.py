@@ -41,6 +41,7 @@ SOURCES = [
     "pretrain.cu",
     "optics.cu",
     "geo_metrics.cu",
+    "jpeg.cu",
 ]
 
 NVCC_FLAGS = [

@@ -89,6 +89,16 @@ class PgCountries(C.Structure):
                 ("index", c_void_p), ("index_bytes", c_size_t), ("entries", c_void_p), ("num_entries", c_int64)]
 
 
+class JpegInfo(C.Structure):
+    _fields_ = [("status", c_int32), ("sof", c_int32), ("precision", c_int32), ("height", c_int32), ("width", c_int32),
+                ("components", c_int32), ("component_id", c_int32 * 3), ("h_samp", c_int32 * 3), ("v_samp", c_int32 * 3),
+                ("quant_table", c_int32 * 3), ("dc_table", c_int32 * 3), ("ac_table", c_int32 * 3),
+                ("restart_interval", c_int32), ("num_segments", c_int32), ("table_mask", c_int32),
+                ("scan_offset", c_int64), ("scan_bytes", c_int64), ("qt", (C.c_uint16 * 64) * 4),
+                ("dc_bits", (C.c_uint8 * 16) * 4), ("ac_bits", (C.c_uint8 * 16) * 4), ("dc_vals", (C.c_uint8 * 256) * 4),
+                ("ac_vals", (C.c_uint8 * 256) * 4)]
+
+
 class GemmProblem(C.Structure):
     _fields_ = [("M", c_int32), ("N", c_int32), ("K", c_int32), ("a", c_void_p), ("lda", c_int32), ("w", c_void_p),
                 ("ldw", c_int32), ("out", c_void_p), ("ldo", c_int32), ("bias", c_void_p), ("epilogue", c_int32),
@@ -160,6 +170,10 @@ SIGNATURES = {
     "pg_preprocess_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
     "pg_preprocess_clip": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int32,
                                      c_void_p]),
+    "pg_jpeg_parse": (c_int32, [c_void_p, c_int64, C.POINTER(JpegInfo)]),
+    "pg_jpeg_workspace_bytes": (c_size_t, [C.POINTER(JpegInfo), c_int32, c_int64]),
+    "pg_jpeg_decode": (c_int32, [c_void_p, c_void_p, C.POINTER(JpegInfo), c_int32, c_void_p, c_void_p, c_size_t, c_void_p,
+                                 c_void_p]),
     "pg_head_loss_grad": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_double,
                                     c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pg_head_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,

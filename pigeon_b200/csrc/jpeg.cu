@@ -1,0 +1,895 @@
+// Baseline JPEG decoding on the GPU, byte-identical to Pillow's `Image.open(f).convert('RGB')` over libjpeg-turbo with
+// its defaults (ISLOW IDCT, fancy upsampling).  Four stages:
+//   host   marker walk (pg_jpeg_parse): frame, tables, restart interval, entropy-coded byte range, restart segments;
+//   kernel 1  Huffman decode, one thread per entropy-coded segment (a restart interval, or the whole scan without DRI):
+//             byte de-stuffing, DC prediction reset per segment, quantised coefficients -> int16 blocks;
+//   kernel 2  dequantise + jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2, 64-bit products like libjpeg's JLONG) + the
+//             post-IDCT range-limit table with its `& RANGE_MASK` wrap -> component planes padded to whole MCUs;
+//   kernel 3  fancy upsampling (jdsample.c h2v1 / h2v2, plain replication when the chroma width is <= 2) fused with
+//             jdcolor.c's fixed-point YCbCr->RGB (SCALEBITS 16) -> uint8 RGB rows in the caller's pg_image destinations.
+// Per-image status: a corrupt image stops its own segments and is not colour-converted; the other images are unaffected.
+// Every read is bounded by the image's own segment, every write by its own planes and destination.
+#include <cuda_runtime.h>
+#include <stdarg.h>
+#include <stdio.h>
+#include <string.h>
+
+#include <algorithm>
+#include <map>
+#include <string>
+#include <vector>
+
+#include "../../include/pigeon_b200.h"
+#include "prof.h"
+#include "tma_host.h"
+
+namespace pg {
+namespace {
+
+constexpr int LOOK_BITS = 9;
+
+struct HuffTbl {                     // libjpeg d_derived_tbl: 9-bit lookahead plus the canonical maxcode / valoffset
+  uint16_t look[1 << LOOK_BITS];     // (code length << 8) | symbol, 0 when the code is longer than LOOK_BITS
+  int32_t maxcode[18];               // largest code of each length, -1 when none; [17] is a sentinel
+  int32_t valoff[17];                // symbol index of the first code of each length, minus that code
+  uint8_t vals[256];
+};
+
+struct Comp {
+  int h, v;                          // sampling factors within the MCU (1 x 1 for a single-component scan)
+  int bw, bh;                        // block grid, padded to whole MCUs
+  int dw, dh;                        // libjpeg downsampled_width / downsampled_height
+  int dc, ac;                        // indices into the batch's Huffman table array
+  long long coef_off;                // first block of this component in the coefficient buffer
+  long long plane_off;               // first byte of this component's plane (bw*8 x bh*8)
+  int16_t q[64];                     // quantisation table in natural order, as libjpeg's ISLOW_MULT_TYPE (short)
+};
+
+struct ImgDesc {
+  int orig;                          // index in the caller's batch (status array)
+  int width, height, ncomp, hmax, vmax, mcux, mcuy, restart_interval;
+  Comp c[3];
+  uint8_t* dst;
+  long long dst_stride;
+};
+
+struct Seg {
+  long long start, end;              // entropy-coded bytes [start, end) in the packed input
+  int img, mcu0, nmcu;
+};
+
+struct PlaneWork {                   // one component plane of one image: IDCT work items [block0, block0 + bw*bh)
+  long long block0;
+  int img, comp;
+};
+
+// entropy-data status codes written by the decode kernel (pg_jpeg_info.status uses the same numbering)
+constexpr int ST_BAD_CODE = PG_JPEG_BAD_CODE, ST_OVERRUN = PG_JPEG_OVERRUN, ST_MARKER = PG_JPEG_UNEXPECTED_MARKER;
+
+inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// jpeg_natural_order: zig-zag index -> natural (row-major) index
+static const uint8_t h_natural[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,
+                                      12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,  7,  14, 21, 28,
+                                      35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
+                                      58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+__constant__ uint8_t c_natural[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,
+                                      12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,  7,  14, 21, 28,
+                                      35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
+                                      58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+
+// ------------------------------------------------------------------------------------------------------------------
+// Host: marker walk
+// ------------------------------------------------------------------------------------------------------------------
+
+struct Why {
+  char* buf;
+  size_t len;
+  int set(int status, const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, len, fmt, ap);
+    va_end(ap);
+    return status;
+  }
+};
+
+inline int be16(const uint8_t* p) { return (p[0] << 8) | p[1]; }
+
+// jdhuff.c jpeg_make_d_derived_tbl: canonical codes; a code that does not fit its length is a bad table.
+bool make_huff(const uint8_t* bits, const uint8_t* vals, bool is_dc, HuffTbl* t) {
+  int count = 0;
+  for (int l = 0; l < 16; ++l) count += bits[l];
+  if (count > 256) return false;
+  if (is_dc)
+    for (int i = 0; i < count; ++i)
+      if (vals[i] > 15) return false;
+  int huffcode[256], huffsize[256];
+  int p = 0;
+  for (int l = 1; l <= 16; ++l)
+    for (int i = 0; i < bits[l - 1]; ++i) huffsize[p++] = l;
+  int code = 0, si = 1;
+  p = 0;
+  while (p < count) {
+    while (p < count && huffsize[p] == si) { huffcode[p++] = code; ++code; }
+    if (code >= (1 << si)) return false;
+    code <<= 1;
+    ++si;
+  }
+  if (!t) return true;
+  memset(t, 0, sizeof(*t));
+  p = 0;
+  for (int l = 1; l <= 16; ++l) {
+    if (bits[l - 1]) {
+      t->valoff[l] = p - huffcode[p];
+      p += bits[l - 1];
+      t->maxcode[l] = huffcode[p - 1];
+    } else {
+      t->maxcode[l] = -1;
+    }
+  }
+  t->maxcode[17] = 0x7fffffff;
+  memcpy(t->vals, vals, count);
+  p = 0;
+  for (int l = 1; l <= LOOK_BITS; ++l)
+    for (int i = 0; i < bits[l - 1]; ++i, ++p) {
+      const int base = huffcode[p] << (LOOK_BITS - l);
+      for (int e = 0; e < (1 << (LOOK_BITS - l)); ++e) t->look[base + e] = (uint16_t)((l << 8) | vals[p]);
+    }
+  return true;
+}
+
+// Walks the entropy-coded data from `pos` to the marker that ends the scan.  Every restart marker ends a segment;
+// `segs` (optional) receives each segment's [start, end).  Returns PG_JPEG_OK and the end-of-scan marker position.
+int walk_scan(const uint8_t* d, int64_t n, int64_t pos, std::vector<std::pair<int64_t, int64_t>>* segs, int* nseg,
+              int64_t* marker_pos, Why* why) {
+  int count = 0;
+  int64_t seg_start = pos;
+  for (;;) {
+    const void* f = pos < n ? memchr(d + pos, 0xFF, (size_t)(n - pos)) : nullptr;
+    if (!f) return why->set(PG_JPEG_NO_EOI, "entropy-coded data runs to the end of the file (no EOI)");
+    const int64_t q = (const uint8_t*)f - d;
+    int64_t r = q + 1;
+    while (r < n && d[r] == 0xFF) ++r;                 // fill bytes
+    if (r >= n) return why->set(PG_JPEG_NO_EOI, "entropy-coded data runs to the end of the file (no EOI)");
+    const int m = d[r];
+    if (m == 0x00) { pos = r + 1; continue; }          // stuffed 0xFF
+    if (m >= 0xD0 && m <= 0xD7) {
+      if ((m - 0xD0) != (count & 7))
+        return why->set(PG_JPEG_BAD_RST, "restart marker RST%d where RST%d was expected", m - 0xD0, count & 7);
+      if (segs) segs->push_back({seg_start, q});
+      ++count;
+      seg_start = pos = r + 1;
+      continue;
+    }
+    if (segs) segs->push_back({seg_start, q});
+    *nseg = count + 1;
+    *marker_pos = q;
+    return PG_JPEG_OK;
+  }
+}
+
+int parse(const uint8_t* d, int64_t n, pg_jpeg_info* info, std::vector<std::pair<int64_t, int64_t>>* segs, Why* why) {
+  memset(info, 0, sizeof(*info));
+  if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return info->status = why->set(PG_JPEG_BAD_HEADER, "no SOI marker");
+  int64_t pos = 2;
+  bool saw_jfif = false, saw_adobe = false, saw_sof = false;
+  int adobe_transform = -1;
+  for (;;) {
+    if (pos >= n) return info->status = why->set(PG_JPEG_BAD_HEADER, "truncated before the scan");
+    if (d[pos] != 0xFF)
+      return info->status = why->set(PG_JPEG_BAD_HEADER, "expected a marker at byte %lld", (long long)pos);
+    while (pos < n && d[pos] == 0xFF) ++pos;            // fill bytes before a marker
+    if (pos >= n) return info->status = why->set(PG_JPEG_BAD_HEADER, "truncated before the scan");
+    const int m = d[pos++];
+    if (m == 0x01) continue;                            // TEM: standalone, ignored as libjpeg does
+    if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x00)
+      return info->status = why->set(PG_JPEG_BAD_HEADER, "marker 0x%02X before the first scan", m);
+    if (pos + 2 > n) return info->status = why->set(PG_JPEG_BAD_HEADER, "truncated marker 0x%02X", m);
+    const int L = be16(d + pos);
+    if (L < 2 || pos + L > n) return info->status = why->set(PG_JPEG_BAD_HEADER, "truncated marker segment 0x%02X", m);
+    const uint8_t* s = d + pos + 2;
+    const int len = L - 2;
+    pos += L;
+    if (m >= 0xC0 && m <= 0xCF && m != 0xC4 && m != 0xC8 && m != 0xCC) {
+      if (saw_sof) return info->status = why->set(PG_JPEG_BAD_HEADER, "second frame header");
+      saw_sof = true;
+      info->sof = m;
+      if (len < 6) return info->status = why->set(PG_JPEG_BAD_HEADER, "short frame header");
+      info->precision = s[0];
+      info->height = be16(s + 1);
+      info->width = be16(s + 3);
+      info->components = s[5];
+      if (m != 0xC0 && m != 0xC1) {
+        const char* kind = m == 0xC2 || m == 0xC6 || m == 0xCA || m == 0xCE ? "progressive"
+                           : m == 0xC3 || m == 0xC7 || m == 0xCB || m == 0xCF ? "lossless"
+                                                                               : "hierarchical or arithmetic";
+        return info->status = why->set(PG_JPEG_UNSUPPORTED, "SOF%d (%s) is not decoded", m - 0xC0, kind);
+      }
+      if (len != 6 + 3 * info->components || info->components < 1)
+        return info->status = why->set(PG_JPEG_BAD_HEADER, "frame header length %d for %d components", len, info->components);
+      if (info->precision != 8)
+        return info->status = why->set(PG_JPEG_UNSUPPORTED, "%d-bit samples are not decoded", info->precision);
+      if (info->height == 0) return info->status = why->set(PG_JPEG_UNSUPPORTED, "height defined by DNL is not decoded");
+      if (info->width == 0) return info->status = why->set(PG_JPEG_BAD_HEADER, "zero width");
+      if (info->components != 1 && info->components != 3)
+        return info->status = why->set(PG_JPEG_UNSUPPORTED, "%d components are not decoded", info->components);
+      for (int c = 0; c < info->components; ++c) {
+        info->component_id[c] = s[6 + 3 * c];
+        info->h_samp[c] = s[7 + 3 * c] >> 4;
+        info->v_samp[c] = s[7 + 3 * c] & 15;
+        info->quant_table[c] = s[8 + 3 * c];
+        if (info->h_samp[c] < 1 || info->h_samp[c] > 4 || info->v_samp[c] < 1 || info->v_samp[c] > 4 ||
+            info->quant_table[c] > 3)
+          return info->status = why->set(PG_JPEG_BAD_HEADER, "bad sampling factor or table of component %d", c);
+      }
+      if (info->components == 3) {
+        const int h = info->h_samp[0], v = info->v_samp[0];
+        const bool luma_ok = (h == 1 && v == 1) || (h == 2 && v == 1) || (h == 2 && v == 2);
+        for (int c = 1; c < 3; ++c)
+          if (!luma_ok || info->h_samp[c] != 1 || info->v_samp[c] != 1)
+            return info->status = why->set(PG_JPEG_UNSUPPORTED, "sampling %dx%d,%dx%d,%dx%d is not decoded", h, v,
+                                           info->h_samp[1], info->v_samp[1], info->h_samp[2], info->v_samp[2]);
+      }
+      continue;
+    }
+    switch (m) {
+      case 0xC4: {                                      // DHT
+        int o = 0;
+        while (o < len) {
+          const int tc = s[o] >> 4, th = s[o] & 15;
+          if (tc > 1 || th > 3 || o + 17 > len) return info->status = why->set(PG_JPEG_BAD_HEADER, "bad DHT segment");
+          int count = 0;
+          for (int i = 0; i < 16; ++i) count += s[o + 1 + i];
+          if (count > 256 || o + 17 + count > len) return info->status = why->set(PG_JPEG_BAD_HEADER, "bad DHT segment");
+          uint8_t* bits = tc ? info->ac_bits[th] : info->dc_bits[th];
+          uint8_t* vals = tc ? info->ac_vals[th] : info->dc_vals[th];
+          memcpy(bits, s + o + 1, 16);
+          memset(vals, 0, 256);
+          memcpy(vals, s + o + 17, count);
+          info->table_mask |= 1 << ((tc ? 8 : 4) + th);
+          o += 17 + count;
+        }
+        break;
+      }
+      case 0xDB: {                                      // DQT, 8- or 16-bit entries
+        int o = 0;
+        while (o < len) {
+          const int pq = s[o] >> 4, tq = s[o] & 15;
+          if (pq > 1 || tq > 3 || o + 1 + 64 * (pq + 1) > len)
+            return info->status = why->set(PG_JPEG_BAD_HEADER, "bad DQT segment");
+          for (int k = 0; k < 64; ++k) info->qt[tq][k] = (uint16_t)(pq ? be16(s + o + 1 + 2 * k) : s[o + 1 + k]);
+          info->table_mask |= 1 << tq;
+          o += 1 + 64 * (pq + 1);
+        }
+        break;
+      }
+      case 0xDD:                                        // DRI
+        if (len != 2) return info->status = why->set(PG_JPEG_BAD_HEADER, "bad DRI segment");
+        info->restart_interval = be16(s);
+        break;
+      case 0xE0:                                        // jdmarker.c examine_app0
+        if (len >= 14 && memcmp(s, "JFIF\0", 5) == 0) saw_jfif = true;
+        break;
+      case 0xEE:                                        // jdmarker.c examine_app14
+        if (len >= 12 && memcmp(s, "Adobe", 5) == 0) { saw_adobe = true; adobe_transform = s[11]; }
+        break;
+      case 0xC8: case 0xCC:
+        return info->status = why->set(PG_JPEG_UNSUPPORTED, "arithmetic coding is not decoded");
+      case 0xDC:
+        return info->status = why->set(PG_JPEG_UNSUPPORTED, "height defined by DNL is not decoded");
+      case 0xDA: {                                      // SOS
+        if (!saw_sof) return info->status = why->set(PG_JPEG_BAD_HEADER, "scan before the frame header");
+        const int ns = len >= 1 ? s[0] : 0;
+        if (len != 4 + 2 * ns || ns < 1) return info->status = why->set(PG_JPEG_BAD_HEADER, "bad SOS segment");
+        if (ns != info->components)
+          return info->status = why->set(PG_JPEG_UNSUPPORTED, "a scan of %d of %d components (more than one scan)", ns,
+                                         info->components);
+        for (int c = 0; c < ns; ++c) {
+          if (s[1 + 2 * c] != info->component_id[c])
+            return info->status = why->set(PG_JPEG_BAD_HEADER, "scan components differ from the frame's");
+          info->dc_table[c] = s[2 + 2 * c] >> 4;
+          info->ac_table[c] = s[2 + 2 * c] & 15;
+          if (info->dc_table[c] > 3 || info->ac_table[c] > 3)
+            return info->status = why->set(PG_JPEG_BAD_HEADER, "bad Huffman table index");
+          if (!(info->table_mask & (1 << info->quant_table[c])) || !(info->table_mask & (16 << info->dc_table[c])) ||
+              !(info->table_mask & (256 << info->ac_table[c])))
+            return info->status = why->set(PG_JPEG_BAD_HEADER, "component %d uses an undefined table", c);
+          if (!make_huff(info->dc_bits[info->dc_table[c]], info->dc_vals[info->dc_table[c]], true, nullptr) ||
+              !make_huff(info->ac_bits[info->ac_table[c]], info->ac_vals[info->ac_table[c]], false, nullptr))
+            return info->status = why->set(PG_JPEG_BAD_HEADER, "invalid Huffman table");
+        }
+        const uint8_t* t = s + 1 + 2 * ns;
+        if (t[0] != 0 || t[1] != 63 || t[2] != 0)
+          return info->status = why->set(PG_JPEG_BAD_HEADER, "spectral selection %d..%d / approximation %d in a sequential scan",
+                                         t[0], t[1], t[2]);
+        // jdapimin.c default_decompress_parms: which 3-component files libjpeg treats as RGB
+        if (info->components == 3 && !saw_jfif) {
+          const bool rgb = saw_adobe ? adobe_transform == 0
+                                     : (info->component_id[0] == 'R' && info->component_id[1] == 'G' &&
+                                        info->component_id[2] == 'B');
+          if (rgb) return info->status = why->set(PG_JPEG_UNSUPPORTED, "RGB colour transform is not decoded");
+        }
+        info->scan_offset = pos;
+        int nseg = 0;
+        int64_t mp = 0;
+        int st = walk_scan(d, n, pos, segs, &nseg, &mp, why);
+        if (st) return info->status = st;
+        info->scan_bytes = mp - pos;
+        info->num_segments = nseg;
+        const int hmax = info->components == 3 ? info->h_samp[0] : 1, vmax = info->components == 3 ? info->v_samp[0] : 1;
+        const long long mcus = (long long)((info->width + 8 * hmax - 1) / (8 * hmax)) * ((info->height + 8 * vmax - 1) / (8 * vmax));
+        const long long want = info->restart_interval ? (mcus + info->restart_interval - 1) / info->restart_interval : 1;
+        if (nseg != want)
+          return info->status = why->set(PG_JPEG_BAD_RST, "%d entropy-coded segments where %lld were expected", nseg, want);
+        // after the scan: only EOI may end the file; another SOS is a second scan
+        int64_t p = mp;
+        for (;;) {
+          while (p < n && d[p] == 0xFF) ++p;
+          if (p >= n) return info->status = why->set(PG_JPEG_NO_EOI, "no EOI after the scan");
+          const int mm = d[p++];
+          if (mm == 0xD9) return info->status = PG_JPEG_OK;
+          if (mm == 0xDA) return info->status = why->set(PG_JPEG_UNSUPPORTED, "more than one scan");
+          if ((mm >= 0xD0 && mm <= 0xD7) || mm == 0x01 || mm == 0x00)
+            return info->status = why->set(PG_JPEG_UNEXPECTED_MARKER, "marker 0x%02X after the scan", mm);
+          if (p + 2 > n || be16(d + p) < 2 || p + be16(d + p) > n)
+            return info->status = why->set(PG_JPEG_NO_EOI, "truncated after the scan");
+          p += be16(d + p);
+          if (p < n && d[p] != 0xFF) return info->status = why->set(PG_JPEG_BAD_HEADER, "garbage after the scan");
+        }
+      }
+      default:
+        if ((m >= 0xE0 && m <= 0xEF) || m == 0xFE) break;   // APPn / COM: skipped
+        return info->status = why->set(PG_JPEG_BAD_HEADER, "unknown marker 0x%02X", m);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Device: entropy decode
+// ------------------------------------------------------------------------------------------------------------------
+
+struct BitReader {
+  const uint8_t* p;
+  const uint8_t* end;
+  uint64_t acc;                      // MSB-aligned
+  int nbits;
+  int zeros;                         // zero bytes fed past the segment end
+  int err;
+
+  __host__ __device__ __forceinline__ void fill() {
+    while (nbits <= 56) {
+      uint32_t c = 0;
+      if (p < end) {
+        c = *p++;
+        if (c == 0xFF) {             // jdhuff.c: skip fill bytes; FF 00 is a data 0xFF, anything else a marker
+          while (p < end && *p == 0xFF) ++p;
+          if (p < end && *p == 0x00) {
+            ++p;
+          } else {
+            err = ST_MARKER;
+            p = end;
+            c = 0;
+          }
+        }
+      } else {
+        ++zeros;
+      }
+      acc |= (uint64_t)c << (56 - nbits);
+      nbits += 8;
+    }
+  }
+  __host__ __device__ __forceinline__ int get(int s) {           // s in 1..16, after fill()
+    const int r = (int)(acc >> (64 - s));
+    acc <<= s;
+    nbits -= s;
+    return r;
+  }
+  __host__ __device__ __forceinline__ bool overrun() const { return zeros * 8 > nbits; }
+};
+
+__host__ __device__ __forceinline__ int huff_decode(BitReader& br, const HuffTbl& t) {
+  const int e = t.look[br.acc >> (64 - LOOK_BITS)];
+  if (e >> 8) {
+    br.acc <<= (e >> 8);
+    br.nbits -= (e >> 8);
+    return e & 0xFF;
+  }
+  int l = LOOK_BITS + 1;
+  int code = (int)(br.acc >> (64 - l));
+  while (code > t.maxcode[l]) {
+    if (++l > 16) { br.err = ST_BAD_CODE; return 0; }
+    code = (int)(br.acc >> (64 - l));
+  }
+  br.acc <<= l;
+  br.nbits -= l;
+  return t.vals[(t.valoff[l] + code) & 0xFF];
+}
+
+__host__ __device__ __forceinline__ int huff_extend(int x, int s) { return x < (1 << (s - 1)) ? x + (int)(~0u << s) + 1 : x; }
+
+// Decodes the MCUs of one entropy-coded segment into int16 blocks (natural order); `blk` is 64 int16 of scratch.
+// Returns 0 or the segment's PG_JPEG_* error.
+__host__ __device__ inline int decode_segment(const uint8_t* __restrict__ bytes, const ImgDesc& im,
+                                              const HuffTbl* __restrict__ tbls, const Seg& sg, int16_t* blk,
+                                              int16_t* __restrict__ coef) {
+#ifdef __CUDA_ARCH__
+  const uint8_t* natural = c_natural;
+#else
+  const uint8_t* natural = h_natural;
+#endif
+  BitReader br{bytes + sg.start, bytes + sg.end, 0, 0, 0, 0};
+  int pred[3] = {0, 0, 0};
+  const int ncomp = im.ncomp;
+  for (int mi = 0; mi < sg.nmcu && !br.err; ++mi) {
+    const int mcu = sg.mcu0 + mi;
+    const int my = mcu / im.mcux, mx = mcu - my * im.mcux;
+    for (int c = 0; c < ncomp && !br.err; ++c) {
+      const Comp& cp = im.c[c];
+      const HuffTbl& dct = tbls[cp.dc];
+      const HuffTbl& act = tbls[cp.ac];
+      for (int bv = 0; bv < cp.v && !br.err; ++bv)
+        for (int bh = 0; bh < cp.h && !br.err; ++bh) {
+          for (int i = 0; i < 64; i += 8) *reinterpret_cast<uint4*>(blk + i) = make_uint4(0, 0, 0, 0);
+          br.fill();
+          int s = huff_decode(br, dct);                 // DC difference, predicted per component within the segment
+          if (s) s = huff_extend(br.get(s), s);
+          pred[c] += s;
+          blk[0] = (int16_t)pred[c];
+          for (int k = 1; k < 64;) {
+            if (br.nbits < 32) br.fill();
+            const int rs = huff_decode(br, act);
+            const int r = rs >> 4;
+            s = rs & 15;
+            if (s) {
+              k += r;
+              if (k > 63) { br.err = ST_BAD_CODE; break; }
+              blk[natural[k]] = (int16_t)huff_extend(br.get(s), s);
+              ++k;
+            } else {
+              if (r != 15) break;
+              k += 16;
+            }
+          }
+          if (br.err) break;
+          const long long b = cp.coef_off + (long long)(my * cp.v + bv) * cp.bw + (mx * cp.h + bh);
+          uint4* o = reinterpret_cast<uint4*>(coef + b * 64);
+          for (int i = 0; i < 8; ++i) o[i] = reinterpret_cast<const uint4*>(blk)[i];
+        }
+    }
+    if (!br.err && br.overrun()) br.err = ST_OVERRUN;
+  }
+  return br.err;
+}
+
+constexpr int ENTROPY_THREADS = 32;
+
+// One thread per entropy-coded segment; `lanes` segments per warp (fewer than 32 when the batch has few segments, so
+// that they spread over the SMs instead of sharing one warp).
+__global__ void __launch_bounds__(ENTROPY_THREADS)
+entropy_kernel(const uint8_t* __restrict__ bytes, const ImgDesc* __restrict__ imgs, const HuffTbl* __restrict__ tbls,
+               const Seg* __restrict__ segs, int nseg, int lanes, int16_t* __restrict__ coef, int* __restrict__ status) {
+  __shared__ __align__(16) int16_t blk_smem[ENTROPY_THREADS][64];
+  const int lane = threadIdx.x;
+  if (lane >= lanes) return;
+  const int si = blockIdx.x * lanes + lane;
+  if (si >= nseg) return;
+  const Seg sg = segs[si];
+  const ImgDesc& im = imgs[sg.img];
+  const int err = decode_segment(bytes, im, tbls, sg, blk_smem[lane], coef);
+  if (err) atomicCAS(status + im.orig, 0, err);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Device: dequantise + jpeg_idct_islow
+// ------------------------------------------------------------------------------------------------------------------
+
+constexpr int CONST_BITS = 13, PASS1_BITS = 2;
+constexpr long long FIX_0_298631336 = 2446, FIX_0_390180644 = 3196, FIX_0_541196100 = 4433, FIX_0_765366865 = 6270,
+                    FIX_0_899976223 = 7373, FIX_1_175875602 = 9633, FIX_1_501321110 = 12299, FIX_1_847759065 = 15137,
+                    FIX_1_961570560 = 16069, FIX_2_053119869 = 16819, FIX_2_562915447 = 20995, FIX_3_072711026 = 25172;
+
+__host__ __device__ __forceinline__ long long descale(long long x, int n) { return (x + (1LL << (n - 1))) >> n; }
+
+// jdmaster.c prepare_range_limit_table, post-IDCT part, indexed by (x & RANGE_MASK)
+__host__ __device__ __forceinline__ uint8_t idct_range_limit(long long v) {
+  const int x = (int)(v & 1023);
+  return (uint8_t)(x < 128 ? x + 128 : x < 512 ? 255 : x < 896 ? 0 : x - 896);
+}
+
+// One 1-D pass of jidctint.c on 8 values in0..in7 (in0 already scaled by the caller); returns the 8 outputs before
+// descaling.
+__host__ __device__ __forceinline__ void idct_1d(long long z0, long long z1in, long long z2in, long long z3in, long long z4in,
+                                        long long z5in, long long z6in, long long z7in, long long out[8]) {
+  // even part
+  long long z2 = z2in, z3 = z6in;
+  long long z1 = (z2 + z3) * FIX_0_541196100;
+  long long tmp2 = z1 + z3 * (-FIX_1_847759065);
+  long long tmp3 = z1 + z2 * FIX_0_765366865;
+  long long tmp0 = (z0 + z4in) * (1LL << CONST_BITS);
+  long long tmp1 = (z0 - z4in) * (1LL << CONST_BITS);
+  const long long tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
+  // odd part
+  tmp0 = z7in; tmp1 = z5in; tmp2 = z3in; tmp3 = z1in;
+  z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2;
+  long long z4 = tmp1 + tmp3;
+  const long long z5 = (z3 + z4) * FIX_1_175875602;
+  tmp0 = tmp0 * FIX_0_298631336;
+  tmp1 = tmp1 * FIX_2_053119869;
+  tmp2 = tmp2 * FIX_3_072711026;
+  tmp3 = tmp3 * FIX_1_501321110;
+  z1 = z1 * (-FIX_0_899976223);
+  z2 = z2 * (-FIX_2_562915447);
+  z3 = z3 * (-FIX_1_961570560);
+  z4 = z4 * (-FIX_0_390180644);
+  z3 += z5; z4 += z5;
+  tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
+  out[0] = tmp10 + tmp3; out[7] = tmp10 - tmp3;
+  out[1] = tmp11 + tmp2; out[6] = tmp11 - tmp2;
+  out[2] = tmp12 + tmp1; out[5] = tmp12 - tmp1;
+  out[3] = tmp13 + tmp0; out[4] = tmp13 - tmp0;
+}
+
+__device__ __forceinline__ int find_plane(const PlaneWork* __restrict__ pw, int np, long long b) {
+  int lo = 0, hi = np - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (pw[mid].block0 <= b) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// Dequantise + IDCT of block `local` of component plane `cp` into its 8x8 pixels.
+__host__ __device__ inline void idct_block(const Comp& cp, long long local, const int16_t* __restrict__ coef,
+                                           uint8_t* __restrict__ planes) {
+  const int by = (int)(local / cp.bw), bx = (int)(local - (long long)by * cp.bw);
+  int16_t in[64];
+  const uint4* src = reinterpret_cast<const uint4*>(coef + (cp.coef_off + local) * 64);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) *reinterpret_cast<uint4*>(in + 8 * i) = src[i];
+  int ws[64];
+#pragma unroll
+  for (int col = 0; col < 8; ++col) {              // pass 1: columns; DEQUANTIZE is a short x short product
+    long long o[8];
+    idct_1d((int)in[col] * (int)cp.q[col], (int)in[8 + col] * (int)cp.q[8 + col], (int)in[16 + col] * (int)cp.q[16 + col],
+            (int)in[24 + col] * (int)cp.q[24 + col], (int)in[32 + col] * (int)cp.q[32 + col],
+            (int)in[40 + col] * (int)cp.q[40 + col], (int)in[48 + col] * (int)cp.q[48 + col],
+            (int)in[56 + col] * (int)cp.q[56 + col], o);
+#pragma unroll
+    for (int r = 0; r < 8; ++r) ws[8 * r + col] = (int)descale(o[r], CONST_BITS - PASS1_BITS);
+  }
+  uint8_t* dst = planes + cp.plane_off + (long long)(by * 8) * (cp.bw * 8) + bx * 8;
+#pragma unroll
+  for (int row = 0; row < 8; ++row) {              // pass 2: rows
+    long long o[8];
+    const int* wr = ws + 8 * row;
+    idct_1d(wr[0], wr[1], wr[2], wr[3], wr[4], wr[5], wr[6], wr[7], o);
+    uint32_t lo = 0, hi = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      lo |= (uint32_t)idct_range_limit(descale(o[i], CONST_BITS + PASS1_BITS + 3)) << (8 * i);
+      hi |= (uint32_t)idct_range_limit(descale(o[4 + i], CONST_BITS + PASS1_BITS + 3)) << (8 * i);
+    }
+    *reinterpret_cast<uint2*>(dst + (long long)row * cp.bw * 8) = make_uint2(lo, hi);
+  }
+}
+
+// One thread per 8x8 block.
+__global__ void __launch_bounds__(128)
+idct_kernel(const ImgDesc* __restrict__ imgs, const PlaneWork* __restrict__ pw, int np, long long nblocks,
+            const int16_t* __restrict__ coef, uint8_t* __restrict__ planes, const int* __restrict__ status) {
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= nblocks) return;
+  const PlaneWork w = pw[find_plane(pw, np, b)];
+  const ImgDesc& im = imgs[w.img];
+  if (status[im.orig]) return;
+  idct_block(im.c[w.comp], b - w.block0, coef, planes);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Device: upsample + colour convert
+// ------------------------------------------------------------------------------------------------------------------
+
+// jdsample.c, one output sample of a chroma component at output column x of output row y
+__host__ __device__ __forceinline__ int chroma_sample(const uint8_t* __restrict__ pl, int stride, int dw, int dh, int hmax,
+                                             int vmax, int x, int y) {
+  if (hmax == 1) return pl[(long long)y * stride + x];
+  const int j = x >> 1;
+  if (vmax == 1) {                                  // h2v1
+    const uint8_t* r = pl + (long long)y * stride;
+    if (dw <= 2) return r[j];
+    if (!(x & 1)) return j == 0 ? r[0] : (r[j] * 3 + r[j - 1] + 1) >> 2;
+    return j == dw - 1 ? r[j] : (r[j] * 3 + r[j + 1] + 2) >> 2;
+  }
+  const int yy = y >> 1;                            // h2v2
+  if (dw <= 2) return pl[(long long)yy * stride + j];
+  const int y2 = (y & 1) ? (yy + 1 < dh ? yy + 1 : dh - 1) : (yy > 0 ? yy - 1 : 0);   // context rows replicate the component's edge rows
+  const uint8_t* r0 = pl + (long long)yy * stride;
+  const uint8_t* r1 = pl + (long long)y2 * stride;
+  const int cs = r0[j] * 3 + r1[j];
+  if (!(x & 1)) return j == 0 ? (cs * 4 + 8) >> 4 : (cs * 3 + (r0[j - 1] * 3 + r1[j - 1]) + 8) >> 4;
+  return j == dw - 1 ? (cs * 4 + 7) >> 4 : (cs * 3 + (r0[j + 1] * 3 + r1[j + 1]) + 7) >> 4;
+}
+
+__host__ __device__ __forceinline__ uint8_t clamp255(int v) { return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v); }
+
+// Output pixel (x, y) of image `im`: luma, upsampled chroma, jdcolor.c ycc_rgb_convert; grayscale is replicated.
+__host__ __device__ inline void color_pixel(const ImgDesc& im, int x, int y, const uint8_t* __restrict__ planes) {
+  uint8_t* o = im.dst + (long long)y * im.dst_stride + 3 * x;
+  const int Y = planes[im.c[0].plane_off + (long long)y * (im.c[0].bw * 8) + x];
+  if (im.ncomp == 1) { o[0] = o[1] = o[2] = (uint8_t)Y; return; }
+  const Comp& cb = im.c[1];
+  const Comp& cr = im.c[2];
+  const int Cb = chroma_sample(planes + cb.plane_off, cb.bw * 8, cb.dw, cb.dh, im.hmax, im.vmax, x, y);
+  const int Cr = chroma_sample(planes + cr.plane_off, cr.bw * 8, cr.dw, cr.dh, im.hmax, im.vmax, x, y);
+  // jdcolor.c build_ycc_rgb_table with SCALEBITS 16, evaluated per sample with the same integer formulas
+  constexpr int SCALEBITS = 16;
+  constexpr long long ONE_HALF = 1LL << (SCALEBITS - 1);
+  constexpr long long F_1_40200 = (long long)(1.40200 * (1L << SCALEBITS) + 0.5),
+                      F_1_77200 = (long long)(1.77200 * (1L << SCALEBITS) + 0.5),
+                      F_0_71414 = (long long)(0.71414 * (1L << SCALEBITS) + 0.5),
+                      F_0_34414 = (long long)(0.34414 * (1L << SCALEBITS) + 0.5);
+  const long long xb = Cb - 128, xr = Cr - 128;
+  const int cr_r = (int)((F_1_40200 * xr + ONE_HALF) >> SCALEBITS);
+  const int cb_b = (int)((F_1_77200 * xb + ONE_HALF) >> SCALEBITS);
+  const long long cr_g = -F_0_71414 * xr;
+  const long long cb_g = -F_0_34414 * xb + ONE_HALF;
+  o[0] = clamp255(Y + cr_r);
+  o[1] = clamp255(Y + (int)((cb_g + cr_g) >> SCALEBITS));
+  o[2] = clamp255(Y + cb_b);
+}
+
+// One thread per output pixel; pix0[i] = first pixel of image i in the flattened batch.
+__global__ void __launch_bounds__(256)
+color_kernel(const ImgDesc* __restrict__ imgs, const long long* __restrict__ pix0, int n, long long npix,
+             const uint8_t* __restrict__ planes, const int* __restrict__ status) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= npix) return;
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (pix0[mid] <= g) lo = mid; else hi = mid - 1;
+  }
+  const ImgDesc& im = imgs[lo];
+  if (status[im.orig]) return;
+  const long long local = g - pix0[lo];
+  const int y = (int)(local / im.width);
+  color_pixel(im, (int)(local - (long long)y * im.width), y, planes);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Host: batch plan
+// ------------------------------------------------------------------------------------------------------------------
+
+struct Plan {
+  std::vector<ImgDesc> imgs;
+  std::vector<HuffTbl> tbls;
+  std::vector<Seg> segs;
+  std::vector<PlaneWork> planes;
+  std::vector<long long> pix0;
+  long long nblocks = 0, plane_bytes = 0, npix = 0;
+  size_t off_imgs = 0, off_tbls = 0, off_segs = 0, off_planes = 0, off_pix0 = 0, meta_bytes = 0;
+  size_t off_bytes = 0, off_meta = 0, off_coef = 0, off_plane = 0, total = 0;
+};
+
+// Sizes every region from the parse results; with `packed` it also fills the tables the kernels read.
+int make_plan(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info* infos, int n, int64_t packed_bytes,
+              const pg_image* dst, Plan* P) {
+  if (n <= 0 || !infos || packed_bytes < 0) { set_last_error("jpeg: bad argument"); return 1; }
+  std::map<std::string, int> tbl_index;
+  long long segs = 0;
+  for (int i = 0; i < n; ++i) {
+    const pg_jpeg_info& in = infos[i];
+    if (in.status != PG_JPEG_OK) continue;
+    if (in.width <= 0 || in.height <= 0 || (in.components != 1 && in.components != 3) || in.num_segments < 1) {
+      set_last_error("jpeg: image %d has an inconsistent pg_jpeg_info", i);
+      return 1;
+    }
+    ImgDesc d;
+    memset(&d, 0, sizeof(d));
+    d.orig = i;
+    d.width = in.width; d.height = in.height; d.ncomp = in.components;
+    d.hmax = in.components == 3 ? in.h_samp[0] : 1;
+    d.vmax = in.components == 3 ? in.v_samp[0] : 1;
+    d.mcux = (in.width + 8 * d.hmax - 1) / (8 * d.hmax);
+    d.mcuy = (in.height + 8 * d.vmax - 1) / (8 * d.vmax);
+    d.restart_interval = in.restart_interval;
+    for (int c = 0; c < d.ncomp; ++c) {
+      Comp& cp = d.c[c];
+      cp.h = d.ncomp == 3 ? in.h_samp[c] : 1;
+      cp.v = d.ncomp == 3 ? in.v_samp[c] : 1;
+      cp.bw = d.mcux * cp.h; cp.bh = d.mcuy * cp.v;
+      cp.dw = (int)(((long long)in.width * cp.h + d.hmax - 1) / d.hmax);
+      cp.dh = (int)(((long long)in.height * cp.v + d.vmax - 1) / d.vmax);
+      cp.coef_off = P->nblocks;
+      cp.plane_off = P->plane_bytes;
+      P->planes.push_back({P->nblocks, (int)P->imgs.size(), c});
+      P->nblocks += (long long)cp.bw * cp.bh;
+      P->plane_bytes += (long long)align_up((size_t)cp.bw * cp.bh * 64, 16);
+      for (int k = 0; k < 64; ++k) cp.q[h_natural[k]] = (int16_t)in.qt[in.quant_table[c]][k];
+      for (int cls = 0; cls < 2; ++cls) {
+        const int th = cls ? in.ac_table[c] : in.dc_table[c];
+        const uint8_t* bits = cls ? in.ac_bits[th] : in.dc_bits[th];
+        const uint8_t* vals = cls ? in.ac_vals[th] : in.dc_vals[th];
+        std::string key(1, (char)cls);
+        key.append((const char*)bits, 16);
+        key.append((const char*)vals, 256);
+        auto it = tbl_index.find(key);
+        int idx;
+        if (it == tbl_index.end()) {
+          idx = (int)P->tbls.size();
+          P->tbls.emplace_back();
+          if (!make_huff(bits, vals, cls == 0, &P->tbls.back())) {
+            set_last_error("jpeg: image %d has an invalid Huffman table", i);
+            return 1;
+          }
+          tbl_index.emplace(key, idx);
+        } else {
+          idx = it->second;
+        }
+        (cls ? cp.ac : cp.dc) = idx;
+      }
+    }
+    if (dst) {
+      if (!dst[i].data || dst[i].height != in.height || dst[i].width != in.width || dst[i].row_stride < 3LL * in.width) {
+        set_last_error("jpeg: destination %d does not match the %dx%d image", i, in.width, in.height);
+        return 1;
+      }
+      d.dst = const_cast<uint8_t*>(dst[i].data);
+      d.dst_stride = dst[i].row_stride;
+    }
+    P->pix0.push_back(P->npix);
+    P->npix += (long long)in.width * in.height;
+    segs += in.num_segments;
+    P->imgs.push_back(d);
+  }
+  const size_t nimg = P->imgs.size();
+  size_t off = 0;
+  P->off_imgs = off; off += align_up(nimg * sizeof(ImgDesc), 256);
+  P->off_tbls = off; off += align_up(P->tbls.size() * sizeof(HuffTbl), 256);
+  P->off_segs = off; off += align_up((size_t)segs * sizeof(Seg), 256);
+  P->off_planes = off; off += align_up(P->planes.size() * sizeof(PlaneWork), 256);
+  P->off_pix0 = off; off += align_up(nimg * sizeof(long long), 256);
+  P->meta_bytes = off;
+  size_t total = 0;
+  P->off_bytes = total; total += align_up((size_t)packed_bytes, 256);
+  P->off_meta = total; total += P->meta_bytes;
+  P->off_coef = total; total += align_up((size_t)P->nblocks * 128, 256);
+  P->off_plane = total; total += align_up((size_t)P->plane_bytes, 256);
+  P->total = total;
+  if (!packed) return 0;
+  // restart segments, found again by the same walk that validated them in pg_jpeg_parse
+  int k = 0;
+  for (int i = 0; i < n; ++i) {
+    const pg_jpeg_info& in = infos[i];
+    if (in.status != PG_JPEG_OK) continue;
+    const ImgDesc& d = P->imgs[k];
+    const int64_t base = offsets[i], len = offsets[i + 1] - offsets[i];
+    if (base < 0 || len < 0 || offsets[i + 1] > packed_bytes || in.scan_offset < 0 || in.scan_bytes < 0 ||
+        in.scan_offset + in.scan_bytes > len) {
+      set_last_error("jpeg: image %d lies outside the packed input", i);
+      return 1;
+    }
+    std::vector<std::pair<int64_t, int64_t>> ranges;
+    char msg[160];
+    Why why{msg, sizeof(msg)};
+    int nseg = 0;
+    int64_t mp = 0;
+    if (walk_scan(packed + base, len, in.scan_offset, &ranges, &nseg, &mp, &why) || nseg != in.num_segments) {
+      set_last_error("jpeg: image %d does not match its pg_jpeg_info", i);
+      return 1;
+    }
+    const int total_mcus = d.mcux * d.mcuy;
+    const int ri = d.restart_interval ? d.restart_interval : total_mcus;
+    for (int s = 0; s < nseg; ++s) {
+      Seg sg;
+      sg.start = base + ranges[s].first;
+      sg.end = base + ranges[s].second;
+      sg.img = k;
+      sg.mcu0 = s * ri;
+      sg.nmcu = std::min(ri, total_mcus - sg.mcu0);
+      P->segs.push_back(sg);
+    }
+    ++k;
+  }
+  return 0;
+}
+
+}  // namespace
+
+int jpeg_parse(const uint8_t* data, int64_t bytes, pg_jpeg_info* info) {
+  if (!info) { set_last_error("pg_jpeg_parse: null info"); return -1; }
+  char msg[200];
+  Why why{msg, sizeof(msg)};
+  msg[0] = 0;
+  const int st = parse(data, bytes, info, nullptr, &why);
+  if (st) set_last_error("%s", msg);
+  return st;
+}
+
+size_t jpeg_workspace_bytes(const pg_jpeg_info* infos, int n, int64_t packed_bytes) {
+  Plan P;
+  if (make_plan(nullptr, nullptr, infos, n, packed_bytes, nullptr, &P)) return 0;
+  return P.total;
+}
+
+int jpeg_decode(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info* infos, int n, const pg_image* dst,
+                void* workspace, size_t workspace_bytes, int32_t* status_out, cudaStream_t stream) {
+  if (!packed || !offsets || !infos || !dst || !status_out || n <= 0) {
+    set_last_error("pg_jpeg_decode: null argument");
+    return 1;
+  }
+  Plan P;
+  if (make_plan(packed, offsets, infos, n, offsets[n], dst, &P)) return 1;
+  if (!workspace || workspace_bytes < P.total || (reinterpret_cast<uintptr_t>(workspace) & 255)) {
+    set_last_error("pg_jpeg_decode: workspace too small (%zu < %zu) or not 256-byte aligned", workspace_bytes, P.total);
+    return 1;
+  }
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  const size_t nimg = P.imgs.size();
+  std::vector<uint8_t> meta(P.meta_bytes, 0);
+  memcpy(meta.data() + P.off_imgs, P.imgs.data(), nimg * sizeof(ImgDesc));
+  memcpy(meta.data() + P.off_tbls, P.tbls.data(), P.tbls.size() * sizeof(HuffTbl));
+  memcpy(meta.data() + P.off_segs, P.segs.data(), P.segs.size() * sizeof(Seg));
+  memcpy(meta.data() + P.off_planes, P.planes.data(), P.planes.size() * sizeof(PlaneWork));
+  memcpy(meta.data() + P.off_pix0, P.pix0.data(), nimg * sizeof(long long));
+  std::vector<int32_t> host_status(n);   // the parse status of skipped images, 0 for the ones the kernels decode
+  for (int i = 0; i < n; ++i) host_status[i] = infos[i].status;
+  cudaError_t e = cudaMemcpyAsync(ws + P.off_bytes, packed, (size_t)offsets[n], cudaMemcpyHostToDevice, stream);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(ws + P.off_meta, meta.data(), P.meta_bytes, cudaMemcpyHostToDevice, stream);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(status_out, host_status.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, stream);
+  if (e != cudaSuccess) { set_last_error("pg_jpeg_decode: upload: %s", cudaGetErrorString(e)); return 1; }
+  if (nimg == 0) return 0;
+  const uint8_t* meta_d = ws + P.off_meta;
+  const ImgDesc* d_imgs = reinterpret_cast<const ImgDesc*>(meta_d + P.off_imgs);
+  const HuffTbl* d_tbls = reinterpret_cast<const HuffTbl*>(meta_d + P.off_tbls);
+  const Seg* d_segs = reinterpret_cast<const Seg*>(meta_d + P.off_segs);
+  const PlaneWork* d_pw = reinterpret_cast<const PlaneWork*>(meta_d + P.off_planes);
+  const long long* d_pix0 = reinterpret_cast<const long long*>(meta_d + P.off_pix0);
+  int16_t* d_coef = reinterpret_cast<int16_t*>(ws + P.off_coef);
+  uint8_t* d_planes = ws + P.off_plane;
+  const int nseg = (int)P.segs.size();
+  int sms = 132;
+  {
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  // one segment per warp until every SM holds 16 warps, then pack lanes
+  const int lanes = (int)std::min<long long>(ENTROPY_THREADS, std::max<long long>(1, (nseg + 16LL * sms - 1) / (16LL * sms)));
+  {
+    ProfScope prof("jpeg_entropy", stream);
+    entropy_kernel<<<(nseg + lanes - 1) / lanes, ENTROPY_THREADS, 0, stream>>>(ws + P.off_bytes, d_imgs, d_tbls, d_segs,
+                                                                                nseg, lanes, d_coef, status_out);
+  }
+  {
+    ProfScope prof("jpeg_idct", stream);
+    idct_kernel<<<(unsigned)((P.nblocks + 127) / 128), 128, 0, stream>>>(d_imgs, d_pw, (int)P.planes.size(), P.nblocks,
+                                                                         d_coef, d_planes, status_out);
+  }
+  {
+    ProfScope prof("jpeg_color", stream);
+    color_kernel<<<(unsigned)((P.npix + 255) / 256), 256, 0, stream>>>(d_imgs, d_pix0, (int)nimg, P.npix, d_planes, status_out);
+  }
+  e = cudaGetLastError();
+  if (e != cudaSuccess) { set_last_error("pg_jpeg_decode launch: %s", cudaGetErrorString(e)); return 1; }
+  return 0;
+}
+
+}  // namespace pg
+
+extern "C" int pg_jpeg_parse(const uint8_t* data_host, int64_t bytes, pg_jpeg_info* info_out) {
+  return pg::jpeg_parse(data_host, bytes, info_out);
+}
+
+extern "C" size_t pg_jpeg_workspace_bytes(const pg_jpeg_info* infos_host, int32_t n, int64_t packed_bytes) {
+  return pg::jpeg_workspace_bytes(infos_host, n, packed_bytes);
+}
+
+extern "C" int pg_jpeg_decode(const uint8_t* packed_host, const int64_t* offsets_host, const pg_jpeg_info* infos_host,
+                              int32_t n, const pg_image* dst_host, void* workspace, size_t workspace_bytes,
+                              int32_t* status_out, void* stream) {
+  return pg::jpeg_decode(packed_host, offsets_host, infos_host, n, dst_host, workspace, workspace_bytes, status_out,
+                         reinterpret_cast<cudaStream_t>(stream));
+}

@@ -1,0 +1,116 @@
+"""Baseline JPEG decoding on the GPU (csrc/jpeg.cu), byte-identical to `np.asarray(PIL.Image.open(f).convert('RGB'))`
+for the files it decodes: what the reference does on the CPU before every CLIPProcessor call
+(dataset_creation/finetune/embed_dataset.py:17-22, dataset_creation/benchmark/benchmark_dataset.py:66-79,
+pretrain_dataset.py:109-161).
+
+    imgs = decode_jpeg([open(p, 'rb').read() for p in paths], 'cuda')     # CUDA uint8 [H, W, 3] views into one arena
+
+The headers are parsed on the host (`parse`); the compressed bytes of the whole batch go to the device in one copy and
+three launches decode them.  Files outside the decoded subset (progressive, 12-bit, CMYK, RGB-transform, other
+sampling layouts) and corrupt files raise `ValueError` naming every such index and its reason.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import List, Sequence, Tuple, Union
+
+import numpy as np
+import torch
+
+from . import _lib
+from ._lib import PigeonB200Error, check, current_stream_ptr, load
+
+OK, UNSUPPORTED, BAD_HEADER, BAD_CODE, OVERRUN, UNEXPECTED_MARKER, BAD_RST, NO_EOI = range(8)
+STATUS_TEXT = {OK: "ok", UNSUPPORTED: "not decoded by this decoder", BAD_HEADER: "truncated or inconsistent header",
+               BAD_CODE: "corrupt entropy data: code missing from its Huffman table",
+               OVERRUN: "corrupt entropy data: a segment ends before its MCUs",
+               UNEXPECTED_MARKER: "corrupt entropy data: marker where data should be",
+               BAD_RST: "corrupt entropy data: wrong restart marker", NO_EOI: "corrupt entropy data: no EOI"}
+
+Encoded = Union[bytes, bytearray, memoryview]
+
+
+class JpegDecodeError(ValueError):
+    """Some files of a batch were not decoded.  `failed` maps each such index to its reason; `images` holds the decoded
+    images of the others (None at the failed indices)."""
+
+    def __init__(self, failed: dict, images: list):
+        super().__init__("JPEG files not decoded: " + "; ".join(f"#{i}: {r}" for i, r in sorted(failed.items())))
+        self.failed = failed
+        self.images = images
+
+
+def parse(data: Encoded) -> Tuple[_lib.JpegInfo, str]:
+    """Host marker walk of one file: its `pg_jpeg_info` and, when its status is not OK, the reason."""
+    lib = load()
+    buf = bytes(data)
+    info = _lib.JpegInfo()
+    st = lib.pg_jpeg_parse(buf, len(buf), C.byref(info))
+    return info, ("" if st == OK else lib.pg_last_error().decode())
+
+
+class JpegDecoder:
+    """Reusable batch decoder: keeps its device workspace and pinned staging buffer between calls."""
+
+    def __init__(self, device: Union[str, torch.device] = "cuda"):
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise PigeonB200Error("JpegDecoder runs on a CUDA device only (no CPU path)")
+        self._lib = load()
+        self._ws = None
+        self._pinned = None        # staging of the compressed bytes; free again once the status has been read back
+
+    def decode(self, files: Sequence[Encoded], infos: Sequence[_lib.JpegInfo] = None) -> List[torch.Tensor]:
+        """files -> CUDA uint8 [H, W, 3] views into one arena (Pillow's `.convert('RGB')` bytes).  `infos` are the
+        `parse` results when the caller already has them.  Raises JpegDecodeError (a ValueError) listing every rejected
+        or corrupt index; the other files of the batch are still decoded."""
+        n = len(files)
+        if n == 0:
+            return []
+        bufs = [memoryview(f).cast("B") for f in files]
+        if infos is None:
+            parsed = [parse(b) for b in bufs]
+            infos = [p[0] for p in parsed]
+            reasons = [p[1] for p in parsed]
+        else:
+            reasons = [STATUS_TEXT.get(i.status, "") for i in infos]
+        info_arr = (_lib.JpegInfo * n)(*infos)
+        offsets = np.zeros(n + 1, dtype=np.int64)
+        offsets[1:] = np.cumsum([len(b) for b in bufs])
+        total = int(offsets[-1])
+        if self._pinned is None or self._pinned.numel() < total:
+            self._pinned = torch.empty(max(total, 1 << 20), dtype=torch.uint8, pin_memory=True)
+        staging = self._pinned.numpy()
+        for i, b in enumerate(bufs):
+            staging[offsets[i]:offsets[i + 1]] = np.frombuffer(b, dtype=np.uint8)
+        sizes = [int(i.height) * int(i.width) * 3 if i.status == OK else 0 for i in infos]
+        starts = np.zeros(n + 1, dtype=np.int64)
+        starts[1:] = np.cumsum([(s + 255) // 256 * 256 for s in sizes])
+        arena = torch.empty(int(starts[-1]), dtype=torch.uint8, device=self.device)
+        base = arena.data_ptr()
+        desc = (_lib.Image * n)()
+        for i, inf in enumerate(infos):
+            if inf.status == OK:
+                desc[i] = _lib.Image(base + int(starts[i]), inf.height, inf.width, 3 * inf.width)
+        need = int(self._lib.pg_jpeg_workspace_bytes(info_arr, n, total))
+        if need == 0:
+            raise PigeonB200Error(f"pg_jpeg_workspace_bytes: {self._lib.pg_last_error().decode()}")
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        status = torch.empty(n, dtype=torch.int32, device=self.device)
+        check(self._lib.pg_jpeg_decode(self._pinned.data_ptr(), offsets.ctypes.data, info_arr, n, desc,
+                                       self._ws.data_ptr(), self._ws.numel(), status.data_ptr(), current_stream_ptr()),
+              "pg_jpeg_decode")
+        st = status.cpu().numpy()                             # synchronises: the pinned buffer is free again
+        images = [arena[int(starts[i]):int(starts[i]) + sizes[i]].view(int(infos[i].height), int(infos[i].width), 3)
+                  if st[i] == OK else None for i in range(n)]
+        failed = {i: (reasons[i] if infos[i].status != OK and reasons[i] else STATUS_TEXT.get(int(s), f"status {int(s)}"))
+                  for i, s in enumerate(st) if s != OK}
+        if failed:
+            raise JpegDecodeError(failed, images)
+        return images
+
+
+def decode_jpeg(files: Sequence[Encoded], device: Union[str, torch.device] = "cuda") -> List[torch.Tensor]:
+    """One-shot `JpegDecoder(device).decode(files)`."""
+    return JpegDecoder(device).decode(files)

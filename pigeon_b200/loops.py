@@ -92,10 +92,26 @@ def raw_image_collate(batch):
     return list(images), torch.as_tensor(index)
 
 
+def encoded_image_collate(batch):
+    """collate_fn for rows of an HF dataset whose `image` column is cast to `Image(decode=False)` (the reference's
+    EmbedDataset rows: data['image'], data['index']): yields (list of encoded files, index).  A row's `bytes` are used,
+    or its `path` is read when `bytes` is None; the model's pre-processor decodes the batch (JPEGs on the GPU)."""
+    files = []
+    for row in batch:
+        im = row['image']
+        data = im.get('bytes')
+        if data is None:
+            with open(im['path'], 'rb') as f:
+                data = f.read()
+        files.append(data)
+    return files, torch.as_tensor([row['index'] for row in batch])
+
+
 def embed_images(loaded_model: Any, dataset, num_workers: int = 0, save_dir: Optional[str] = 'data/landmark_embeddings',
                  collate_fn=None):
     """reference preprocessing/embed.py:45-83.  `dataset` maps split name -> dataset yielding (pixels, index); with
-    `collate_fn=raw_image_collate` the items may be raw uint8 images instead of CPU-pre-processed tensors."""
+    `collate_fn=raw_image_collate` the items may be raw uint8 images instead of CPU-pre-processed tensors, with
+    `collate_fn=encoded_image_collate` rows of encoded images."""
     loaded_model.eval()
     for split in ('train', 'val', 'test'):
         if split not in dataset:

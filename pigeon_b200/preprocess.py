@@ -5,15 +5,21 @@ dataset_creation/benchmark/benchmark_dataset.py:100-104): raw uint8 RGB images g
 
     proc = ClipImageProcessor()                       # openai/clip-vit-large-patch14-336 settings
     px = proc(images=[pil_or_ndarray, ...], return_tensors='pt')['pixel_values']    # CUDA [n, 3, 336, 336]
+
+Images may also be encoded files (`bytes` / `bytearray` / `memoryview`).  Baseline JPEGs are decoded on the GPU
+(pigeon_b200.jpeg, one decode launch sequence per call); every other encoded file (PNG, progressive JPEG, anything the
+JPEG parser does not decode) is decoded by Pillow on the host, the reference's own decoder, so the pixels are the same
+either way.  `gpu_decoded` / `host_decoded` count the two routes.  A JPEG with corrupt entropy-coded data raises.
 """
 from __future__ import annotations
 
+import io
 from typing import List, Sequence, Union
 
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, jpeg
 from ._lib import PigeonB200Error, check, current_stream_ptr, load
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
@@ -33,6 +39,17 @@ def _to_u8_rgb(img) -> np.ndarray:
     return np.ascontiguousarray(img)
 
 
+def route_encoded(data) -> tuple:
+    """('gpu', info) for a file the GPU JPEG decoder takes, ('host', info) for one Pillow decodes on the host (PNG,
+    progressive JPEG, anything else the parser does not decode); ValueError for a JPEG with corrupt entropy data."""
+    info, reason = jpeg.parse(data)
+    if info.status == jpeg.OK:
+        return "gpu", info
+    if info.status in (jpeg.UNSUPPORTED, jpeg.BAD_HEADER):
+        return "host", info
+    raise ValueError(f"corrupt JPEG: {reason}")
+
+
 class ClipImageProcessor:
     """Call-compatible with the way the reference uses `CLIPProcessor` for images: `proc(images=..., return_tensors='pt')`
     returns a dict with 'pixel_values' (here a CUDA tensor).  `dtype=torch.float16` writes the tower's input type directly."""
@@ -50,6 +67,9 @@ class ClipImageProcessor:
         self.dtype = dtype
         self._lib = load()
         self._ws = None
+        self._jpeg = None
+        self.gpu_decoded = 0
+        self.host_decoded = 0
 
     def preprocess_device(self, images_u8: List[torch.Tensor]) -> torch.Tensor:
         """images_u8: CUDA uint8 tensors [H, W, 3] (any sizes, rows may be strided) -> [n, 3, size, size]."""
@@ -75,11 +95,31 @@ class ClipImageProcessor:
             raise ValueError("You have to specify images.")
         if not isinstance(images, (list, tuple)):
             images = [images]
-        dev = []
-        for img in images:
+        dev = [None] * len(images)
+        gpu_idx, gpu_files, gpu_infos = [], [], []
+        for i, img in enumerate(images):
             if isinstance(img, torch.Tensor) and img.is_cuda:
-                dev.append(img)
+                dev[i] = img
                 continue
+            if isinstance(img, (bytes, bytearray, memoryview)):
+                try:
+                    route, info = route_encoded(img)
+                except ValueError as e:
+                    raise ValueError(f"image {i}: {e}") from None
+                if route == "gpu":
+                    gpu_idx.append(i)
+                    gpu_files.append(img)
+                    gpu_infos.append(info)
+                    continue
+                from PIL import Image
+                img = Image.open(io.BytesIO(bytes(img)))
+                self.host_decoded += 1
             a = torch.from_numpy(_to_u8_rgb(img))
-            dev.append(a.pin_memory().to(self.device, non_blocking=True))
+            dev[i] = a.pin_memory().to(self.device, non_blocking=True)
+        if gpu_files:
+            if self._jpeg is None:
+                self._jpeg = jpeg.JpegDecoder(self.device)
+            for i, t in zip(gpu_idx, self._jpeg.decode(gpu_files, gpu_infos)):
+                dev[i] = t
+            self.gpu_decoded += len(gpu_files)
         return {"pixel_values": self.preprocess_device(dev)}

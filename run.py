@@ -2,7 +2,7 @@
 """Entry points of the hot path with the reference's CLI (run.py:21-93): `embed`, `evaluate` and `finetune`.
 
     python run.py evaluate HEAD.model -l DATASET_DIR [-b BASE.model] [--yfcc] [--metrics]
-    python run.py embed CLIP.model -l DATASET_DIR
+    python run.py embed CLIP.model -l DATASET_DIR                                                # image column + index
     python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading]     # tower + head (run.py:165-169)
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
 
@@ -25,7 +25,7 @@ import torch
 
 from pigeon_b200 import CLIPEmbedding, ProtoRefiner, SuperGuessr
 from pigeon_b200 import config as cfg
-from pigeon_b200.loops import embed_images, evaluate_model
+from pigeon_b200.loops import embed_images, encoded_image_collate, evaluate_model
 
 logger = logging.getLogger('run')
 
@@ -117,7 +117,11 @@ def main(argv=None):
                            metrics=metrics_fn(args))                                                          # run.py:169
     elif args.mode == 'embed':
         model = CLIPEmbedding(args.name, load_checkpoint=True, panorama=not args.yfcc)    # run.py:126-129
-        embed_images(model, dataset)
+        # EmbedDataset semantics (embed_dataset.py:17-22): data['image'] and data['index'] of each split; the files stay
+        # encoded until the GPU decodes them
+        from datasets import Image
+        splits = {k: v.cast_column('image', Image(decode=False)) for k, v in dataset.items()}
+        embed_images(model, splits, collate_fn=encoded_image_collate)
     else:
         split = dataset['test'] if 'test' in dataset else dataset[list(dataset.keys())[-1]]
         print(evaluate(args.name, split.with_format('torch'), args.yfcc, args.landmarks, base_model=args.base,
