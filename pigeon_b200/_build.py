@@ -23,6 +23,7 @@ SOURCES = [
     "tma_host.cu",
     "gemm_wgmma.cu",
     "gemm_pingpong.cu",
+    "gemm_wide.cu",
     "attention_wgmma.cu",
     "nccl_gather.cu",
     "vit_misc.cu",

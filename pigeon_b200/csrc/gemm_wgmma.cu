@@ -15,12 +15,14 @@
 //               (each warp 32 rows: bias / activation / residual -> global)
 //   warp 4      TMA producer (one lane): global -> 4-stage smem ring, 128B swizzle; it runs ahead into the next tile
 //               while the warpgroup is in its epilogue
-// K-major problems run the ping-pong kernel of gemm_pingpong.cu (same tiles and MMAs, two consumer warpgroups) unless
-// pg_gemm_set_schedule(1) selects this one; MN-major operands always run here.  launch<EPI> below checks the problem and
-// builds the tensor maps for both.
+// K-major problems run the 128 x 256 kernel of gemm_wide.cu (fp16-output epilogues whose output rows suit a TMA store)
+// or the ping-pong kernel of gemm_pingpong.cu (same tiles and MMAs as this one, two consumer warpgroups), unless
+// pg_gemm_set_schedule(1) selects this one for all of them or (2) the ping-pong kernel; MN-major operands always run here.
+// launch<EPI> below checks the problem and builds the tensor maps for all three.
 #include "gemm.h"
 #include "gemm_epilogue.cuh"
 #include "gemm_pingpong.h"
+#include "gemm_wide.h"
 #include "ptx.cuh"
 #include "prof.h"
 #include "tma_host.h"
@@ -30,22 +32,23 @@
 
 namespace pg {
 
-// Process-wide kernel choice (pg_gemm_set_schedule).  It exists so that tests can take the single-warpgroup kernel as the
-// bit-exact reference of the ping-pong kernel and a benchmark can compare the two in one process; it is not a tuning knob.
-// PG_GEMM_SCHEDULE=1 only sets the initial value, once.
+// Process-wide kernel choice (pg_gemm_set_schedule): 0 = automatic, 1 = the single-warpgroup kernel for every problem,
+// 2 = the ping-pong kernel for every K-major problem.  It exists so that tests can take the single-warpgroup and the
+// ping-pong kernels as the bit-exact references of the kernels that replace them, and a benchmark can compare them in one
+// process; it is not a tuning knob.  PG_GEMM_SCHEDULE=1 or 2 only sets the initial value, once.
 static std::atomic<int> g_gemm_schedule{-1};
 static int gemm_schedule() {
   int v = g_gemm_schedule.load(std::memory_order_relaxed);
   if (v < 0) {
     const char* e = getenv("PG_GEMM_SCHEDULE");
-    v = (e && e[0] == '1') ? 1 : 0;
+    v = (e && (e[0] == '1' || e[0] == '2')) ? e[0] - '0' : 0;
     g_gemm_schedule.store(v, std::memory_order_relaxed);
   }
   return v;
 }
 
 int gemm_set_schedule(int mode) {
-  if (mode != 0 && mode != 1) { set_last_error("pg_gemm_set_schedule: mode %d not in {0, 1}", mode); return 1; }
+  if (mode < 0 || mode > 2) { set_last_error("pg_gemm_set_schedule: mode %d not in {0, 1, 2}", mode); return 1; }
   g_gemm_schedule.store(mode, std::memory_order_relaxed);
   return 0;
 }
@@ -196,13 +199,18 @@ int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& 
 template <int EPI>
 int launch(const GemmProblem& p, int num_sms, cudaStream_t stream) {
   constexpr bool f16_out = EpiTraits<EPI>::kF16Out || EPI == EPI_BF16_DGELU;   // 2-byte output elements
+  const int sched = gemm_schedule();
+  // The 128 x 256 kernel stores its output with TMA: row pitch a multiple of 16 bytes (`out` is 16-byte aligned, checked
+  // by gemm_f16).  Otherwise the problem takes the ping-pong kernel, which gives the same bits.
+  const bool wide = gemm_wide_epilogue(EPI) && !p.mn_major && sched == 0 && p.ldo % 8 == 0;
+  const int block_n = wide ? kWideBlockN : BLOCK_N;
   CUtensorMap ta, tb;
   if (p.mn_major) {   // tensors are [K, M] and [K, N]; box = 64 contraction rows x 64 columns
     if (make_tmap_f16_2d(&ta, p.a, p.K, p.M, p.lda, BLOCK_K, 64)) return 1;
     if (make_tmap_f16_2d(&tb, p.w, p.K, p.N, p.ldw, BLOCK_K, 64)) return 1;
   } else {
     if (make_tmap_f16_2d(&ta, p.a, p.M, p.K, p.lda, BLOCK_M, BLOCK_K)) return 1;
-    if (make_tmap_f16_2d(&tb, p.w, p.N, p.K, p.ldw, BLOCK_N, BLOCK_K)) return 1;
+    if (make_tmap_f16_2d(&tb, p.w, p.N, p.K, p.ldw, block_n, BLOCK_K)) return 1;
   }
   GemmArgs a;
   a.M = p.M; a.N = p.N; a.K = p.K; a.out = p.out; a.ldo = p.ldo; a.bias = p.bias;
@@ -227,16 +235,22 @@ int launch(const GemmProblem& p, int num_sms, cudaStream_t stream) {
     }
     a.stats_slots = p.K / 128;
   }
-  const int m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M, n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
+  const int m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M, n_blocks = (p.N + block_n - 1) / block_n;
   const int tiles = m_blocks * n_blocks;
   const int grid = tiles < num_sms ? tiles : num_sms;
   static const char* const kNames[] = {"gemm_f16_bias", "gemm_f16_bias_qgelu", "gemm_f32_bias_resid", "gemm_f32_bias", "gemm_f32_rowmap",
                                        "gemm_bf16_dgelu", "gemm_f16_bias_qgelu_save", "gemm_f32_bias_resid_stats", "gemm_f16_ln_bias",
                                        "gemm_f16_ln_bias_qgelu"};
   ProfScope prof(kNames[EPI], stream);
-  // K-major problems go to the ping-pong kernel (gemm_pingpong.cu): same tiles and MMAs, so the same bits, with each
-  // tile's epilogue overlapping the next tile's MMAs.  MN-major operands (pg_gemm_tn) stay on gemm_f16_kernel.
-  if (!p.mn_major && gemm_schedule() == 0) return gemm_pingpong_launch(EPI, p.operand_bf16 != 0, ta, tb, a, grid, stream);
+  // fp16-output problems go to the 128 x 256 kernel (gemm_wide.cu), other K-major ones to the ping-pong kernel
+  // (gemm_pingpong.cu); both sum the same products in the same order as gemm_f16_kernel, so the same bits.  MN-major
+  // operands (pg_gemm_tn) stay on gemm_f16_kernel.
+  if (wide) {
+    CUtensorMap tout;   // fp16 [M, N] with row pitch ldo, stored in 64 x 64 boxes
+    if (make_tmap_f16_2d(&tout, p.out, p.M, p.N, p.ldo, 64, 64)) return 1;
+    return gemm_wide_launch(EPI, p.operand_bf16 != 0, ta, tb, tout, a, grid, stream);
+  }
+  if (!p.mn_major && sched != 1) return gemm_pingpong_launch(EPI, p.operand_bf16 != 0, ta, tb, a, grid, stream);
   if (p.mn_major) return p.operand_bf16 ? launch_kernel<EPI, true, true>(ta, tb, a, grid, stream) : launch_kernel<EPI, false, true>(ta, tb, a, grid, stream);
   return p.operand_bf16 ? launch_kernel<EPI, true, false>(ta, tb, a, grid, stream) : launch_kernel<EPI, false, false>(ta, tb, a, grid, stream);
 }

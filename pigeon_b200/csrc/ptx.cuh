@@ -111,6 +111,25 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// 2-D tiled store shared -> global in the issuing thread's bulk async-group; elements past the tensor's bounds are not
+// written.  The shared source must be made visible to the async proxy first (fence_proxy_async_smem by every writer).
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// Waits until at most N bulk async-groups of this thread are still reading their shared-memory source.
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// Waits until at most N bulk async-groups of this thread are incomplete (their writes done).
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+
 // Explicit shared-window accesses (a pointer that went through integer alignment arithmetic is "generic" to the compiler,
 // which then emits LD.E / ST.E with their address-space check instead of LDS / STS).
 __device__ __forceinline__ float4 lds_f4(uint32_t saddr) {
@@ -129,6 +148,9 @@ __device__ __forceinline__ float lds_f1(uint32_t saddr) {
 }
 __device__ __forceinline__ void sts_f1(uint32_t saddr, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(saddr), "f"(v) : "memory");
+}
+__device__ __forceinline__ void sts_u1(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
 }
 __device__ __forceinline__ uint4 lds_u4(uint32_t saddr) {
   uint4 v;

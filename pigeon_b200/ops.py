@@ -35,7 +35,8 @@ def gemm_f16(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, epilog
 
 
 def gemm_set_schedule(mode: int) -> None:
-    """Kernel of every K-major GEMM, process-wide: 0 = automatic (ping-pong), 1 = the single-warpgroup kernel (same bits)."""
+    """Kernel of every K-major GEMM, process-wide: 0 = automatic (128 x 256 for the fp16-output projections, else
+    ping-pong), 1 = the single-warpgroup kernel, 2 = the ping-pong kernel (all the same bits)."""
     check(load().pg_gemm_set_schedule(int(mode)), "pg_gemm_set_schedule")
 
 

@@ -1,14 +1,15 @@
-"""GEMM schedules on one GPU: the ping-pong kernel (schedule 0, the default) against the single-warpgroup kernel
-(schedule 1, pg_gemm_set_schedule).  Writes one JSON file, <out>/gemm_bench.json, with the card's name, power limit and
-SM clocks (read-only nvidia-smi queries) beside the numbers.
+"""GEMM schedules on one GPU: the automatic choice (schedule 0, the default: the 128 x 256 kernel for the fp16-output
+projections, ping-pong for the rest) against the ping-pong kernel for every K-major GEMM (schedule 2,
+pg_gemm_set_schedule).  Writes one JSON file, <out>/gemm_bench.json, with the card's name, power limit and SM clocks
+(read-only nvidia-smi queries) beside the numbers.
 
   1. per GEMM family at the real shapes: VitEngine.forward on --views views of ViT-L/14-336 (LayerNorm folded), device
      time per family from the library's launch events, both schedules alternating, --rounds rounds each;
-  2. K-sweep: M = 590 848 (1024 views x 577 tokens), N in {1024, 3072}, K in {256 .. 4096}, EPI_F32_BIAS and EPI_F16_BIAS,
-     both schedules, fitted to t = a + b K: b gives the mainloop rate, a the per-tile fixed cost (epilogue, fill, drain);
-     torch.matmul (cuBLAS) at the same shapes as a reference point on the same card;
+  2. K-sweep: M = 590 848 (1024 views x 577 tokens), N in {1024, 3072}, K in {256 .. 4096}, EPI_F16_BIAS and
+     EPI_F16_BIAS_QGELU, both schedules, fitted to t = a + b K: b gives the mainloop rate, a the per-tile fixed cost
+     (epilogue, fill, drain); torch.matmul (cuBLAS) at the same shapes as a reference point on the same card;
   3. --bench-ab: bench.py --steps 10 --warmup 3 --no-cpu-baseline --dump-outputs as a subprocess, 3 times with
-     PG_GEMM_SCHEDULE=1 and 3 times without, alternating; every dumped array of the two schedules compared bit for bit.
+     PG_GEMM_SCHEDULE=2 and 3 times without, alternating; every dumped array of the two schedules compared bit for bit.
 
 usage: python tools/gemm_bench.py [--out DIR] [--bench-ab] [--skip-families] [--skip-sweep]"""
 from __future__ import annotations
@@ -29,6 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 TOKENS = 577
+SCHEDULES = (0, 2)   # the automatic choice, and its reference: the ping-pong kernel for every K-major GEMM
 SWEEP_K = (256, 512, 1024, 2048, 4096)
 
 
@@ -69,13 +71,13 @@ def families(views, rounds):
             "gemm_f16_ln_bias_qgelu": 2 * M * I * H * L,                        # fc1
             "out_proj+fc2": 2 * M * H * H * L + 2 * M * H * I * L,              # gemm_f32_bias_resid(_stats)
             "gemm_f32_rowmap": 2 * views * (TOKENS - 1) * H * patch_k}          # patch embedding
-    res = {0: [], 1: []}
-    for sched in (0, 1):                      # warm-up: module load, tensor maps, attributes
+    res = {s: [] for s in SCHEDULES}
+    for sched in SCHEDULES:                   # warm-up: module load, tensor maps, attributes
         ops.gemm_set_schedule(sched)
         eng.forward(px)
     torch.cuda.synchronize()
     for _ in range(rounds):
-        for sched in (0, 1):
+        for sched in SCHEDULES:
             ops.gemm_set_schedule(sched)
             lib.pg_profile_begin()
             eng.forward(px)
@@ -122,14 +124,14 @@ def sweep(reps=5):
     for N in (1024, 3072):
         w = (torch.randn(N, Kmax, device="cuda", generator=g) * 0.03).half()
         bias = torch.randn(N, device="cuda", generator=g)
-        for epi, name, dt in ((3, "EPI_F32_BIAS", torch.float32), (0, "EPI_F16_BIAS", torch.float16)):
-            o = torch.empty(M, N, device="cuda", dtype=dt)
-            for sched in (0, 1):
+        for epi, name in ((0, "EPI_F16_BIAS"), (1, "EPI_F16_BIAS_QGELU")):
+            o = torch.empty(M, N, device="cuda", dtype=torch.float16)
+            for sched in SCHEDULES:
                 ops.gemm_set_schedule(sched)
                 ts = [timed(lambda: check(lib.pg_gemm_f16(ptr(a), Kmax, ptr(w), Kmax, ptr(o), N, ptr(bias), M, N, K, epi,
                                                           current_stream_ptr()), "pg_gemm_f16")) for K in SWEEP_K]
                 b, a0 = np.polyfit(np.array(SWEEP_K, dtype=float), np.array(ts), 1)
-                tiles = (M // 128) * (N // 128)
+                tiles = (M // 128) * (N // (256 if sched == 0 else 128))
                 out["configs"][f"N{N}_{name}_schedule{sched}"] = {
                     "ms": ts, "tflops": [2 * M * N * K / (t / 1e3) / 1e12 for K, t in zip(SWEEP_K, ts)],
                     "fit_ms_intercept": a0, "fit_ms_per_k": b,
@@ -151,16 +153,16 @@ def sweep(reps=5):
 
 def bench_ab(runs=3):
     """bench.py under both schedules, alternating; outputs compared bit for bit."""
-    res = {"schedule_0": [], "schedule_1": []}
-    dirs = {0: [], 1: []}
+    res = {f"schedule_{s}": [] for s in SCHEDULES}
+    dirs = {s: [] for s in SCHEDULES}
     tmp = tempfile.mkdtemp(prefix="gemm_bench_ab_")
     for r in range(runs):
-        for sched in (1, 0):
+        for sched in SCHEDULES[::-1]:
             d = os.path.join(tmp, f"s{sched}_r{r}")
             env = dict(os.environ)
             env.pop("PG_GEMM_SCHEDULE", None)
-            if sched == 1:
-                env["PG_GEMM_SCHEDULE"] = "1"
+            if sched != 0:
+                env["PG_GEMM_SCHEDULE"] = str(sched)
             p = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", "10", "--warmup", "3",
                                 "--no-cpu-baseline", "--dump-outputs", d], capture_output=True, text=True, env=env, cwd=ROOT)
             line = [l for l in p.stdout.splitlines() if l.startswith("{")]
@@ -170,15 +172,16 @@ def bench_ab(runs=3):
             res[f"schedule_{sched}"].append(j)
             dirs[sched].append(d)
     same = {}
-    for name in sorted(os.listdir(dirs[1][0])):
-        ref = np.load(os.path.join(dirs[1][0], name))
-        same[name] = all(np.array_equal(np.load(os.path.join(d, name)), ref) for d in dirs[0] + dirs[1])
-    v = {s: [j["value"] for j in res[f"schedule_{s}"]] for s in (0, 1)}
-    summary = {"images_per_s": {f"schedule_{s}": spread(v[s]) for s in (0, 1)},
-               "speedup_median": statistics.median(v[0]) / statistics.median(v[1]),
-               "every_new_run_faster": min(v[0]) > max(v[1]),
+    ref_dirs = dirs[SCHEDULES[1]]
+    for name in sorted(os.listdir(ref_dirs[0])):
+        ref = np.load(os.path.join(ref_dirs[0], name))
+        same[name] = all(np.array_equal(np.load(os.path.join(d, name)), ref) for d in dirs[0] + ref_dirs)
+    v = {s: [j["value"] for j in res[f"schedule_{s}"]] for s in SCHEDULES}
+    summary = {"images_per_s": {f"schedule_{s}": spread(v[s]) for s in SCHEDULES},
+               "speedup_median": statistics.median(v[0]) / statistics.median(v[SCHEDULES[1]]),
+               "every_new_run_faster": min(v[0]) > max(v[SCHEDULES[1]]),
                "outputs_bit_identical": same, "all_outputs_bit_identical": all(same.values()),
-               "parity_ok_all_runs": all(j["parity_check"]["ok"] for s in (0, 1) for j in res[f"schedule_{s}"]),
+               "parity_ok_all_runs": all(j["parity_check"]["ok"] for s in SCHEDULES for j in res[f"schedule_{s}"]),
                "runs": res}
     return summary
 
@@ -209,7 +212,9 @@ def main():
         json.dump(result, f, indent=1)
     brief = {k: v for k, v in result.get("bench_ab", {}).items() if k != "runs"}
     print(json.dumps({"gpu": result["gpu"], "bench_ab": brief,
-                      "families_gemm_total": {s: result["families"][s]["gemm_total"] for s in ("schedule_0", "schedule_1")}
+                      "families": {f"schedule_{s}": {k: (round(v["ms"]["median"], 2), v["tflops_median"] and round(v["tflops_median"]))
+                                                     for k, v in result["families"][f"schedule_{s}"].items()}
+                                   for s in SCHEDULES}
                       if "families" in result else None}))
 
 
