@@ -498,8 +498,8 @@ enum {
 int pg_gemm_f16(const void* a, int32_t lda, const void* w, int32_t ldw, void* out, int32_t ldo, const float* bias,
                 int32_t M, int32_t N, int32_t K, int32_t epilogue, void* stream);
 /* Kernel of every K-major GEMM (pg_gemm_f16, pg_gemm_ex and the towers), process-wide: 0 = automatic (default; the 128 x 256
- * kernel for the fp16-output epilogues without side outputs when ldo % 8 == 0, else the ping-pong kernel, whose epilogues
- * overlap the next tile's MMAs), 1 = the single-warpgroup kernel, 2 = the ping-pong kernel.  All give the same bits; the
+ * kernel for the fp16-output epilogues without side outputs and the fp32 residual epilogues when ldo % 8 == 0, else the
+ * ping-pong kernel, whose epilogues overlap the next tile's MMAs), 1 = the single-warpgroup kernel, 2 = the ping-pong kernel.  All give the same bits; the
  * switch exists for tests and A/B benchmarks, not for tuning.  PG_GEMM_SCHEDULE=1 or 2 only sets the initial value, once. */
 int pg_gemm_set_schedule(int32_t mode);
 /* pg_gemm_f16 with bf16 operands (operand_bf16 != 0: BOTH a and w are bf16 — the tensor cores reject mixed pairs) and,

@@ -24,6 +24,7 @@ SOURCES = [
     "gemm_wgmma.cu",
     "gemm_pingpong.cu",
     "gemm_wide.cu",
+    "gemm_wide_resid.cu",
     "attention_wgmma.cu",
     "nccl_gather.cu",
     "vit_misc.cu",

@@ -48,8 +48,8 @@ struct GemmProblem {
 // Enqueues the GEMM on `stream`. Returns 0 on success; on failure the message is in pg::last_error().
 int gemm_f16(const GemmProblem& p, int num_sms, cudaStream_t stream);
 
-// Kernel choice for K-major problems, process-wide: 0 = automatic (the 128 x 256 kernel for the fp16-output epilogues, else
-// the ping-pong kernel), 1 = the single-warpgroup kernel, 2 = the ping-pong kernel.
+// Kernel choice for K-major problems, process-wide: 0 = automatic (the 128 x 256 kernel for the fp16-output and fp32 residual
+// epilogues, else the ping-pong kernel), 1 = the single-warpgroup kernel, 2 = the ping-pong kernel.
 int gemm_set_schedule(int mode);
 
 }  // namespace pg

@@ -1,5 +1,5 @@
 // Launcher of the ping-pong GEMM kernel (gemm_pingpong.cu); gemm_wgmma.cu validates the problem, builds the tensor maps and
-// picks this kernel, the 128 x 256 one (gemm_wide.cu) or its own single-warpgroup one.
+// picks this kernel, the 128 x 256 one (gemm_wide.cuh) or its own single-warpgroup one.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

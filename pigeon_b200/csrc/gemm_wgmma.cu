@@ -15,9 +15,10 @@
 //               (each warp 32 rows: bias / activation / residual -> global)
 //   warp 4      TMA producer (one lane): global -> 4-stage smem ring, 128B swizzle; it runs ahead into the next tile
 //               while the warpgroup is in its epilogue
-// K-major problems run the 128 x 256 kernel of gemm_wide.cu (fp16-output epilogues whose output rows suit a TMA store)
-// or the ping-pong kernel of gemm_pingpong.cu (same tiles and MMAs as this one, two consumer warpgroups), unless
-// pg_gemm_set_schedule(1) selects this one for all of them or (2) the ping-pong kernel; MN-major operands always run here.
+// K-major problems run the 128 x 256 kernel of gemm_wide.cuh (fp16-output and fp32 residual epilogues whose output rows
+// suit a TMA store) or the ping-pong kernel of gemm_pingpong.cu (same tiles and MMAs as this one, two consumer
+// warpgroups), unless pg_gemm_set_schedule(1) selects this one for all of them or (2) the ping-pong kernel; MN-major
+// operands always run here.
 // launch<EPI> below checks the problem and builds the tensor maps for all three.
 #include "gemm.h"
 #include "gemm_epilogue.cuh"
@@ -200,8 +201,9 @@ template <int EPI>
 int launch(const GemmProblem& p, int num_sms, cudaStream_t stream) {
   constexpr bool f16_out = EpiTraits<EPI>::kF16Out || EPI == EPI_BF16_DGELU;   // 2-byte output elements
   const int sched = gemm_schedule();
-  // The 128 x 256 kernel stores its output with TMA: row pitch a multiple of 16 bytes (`out` is 16-byte aligned, checked
-  // by gemm_f16).  Otherwise the problem takes the ping-pong kernel, which gives the same bits.
+  // The 128 x 256 kernel stores its output (and loads the residual, stores the fp16 copy) with TMA: row pitch a multiple of
+  // 16 bytes for the fp16 output and copy (`out`, `resid` and `aux` are 16-byte aligned, checked by gemm_f16 and below).
+  // Otherwise the problem takes the ping-pong kernel, which gives the same bits.
   const bool wide = gemm_wide_epilogue(EPI) && !p.mn_major && sched == 0 && p.ldo % 8 == 0;
   const int block_n = wide ? kWideBlockN : BLOCK_N;
   CUtensorMap ta, tb;
@@ -242,13 +244,25 @@ int launch(const GemmProblem& p, int num_sms, cudaStream_t stream) {
                                        "gemm_bf16_dgelu", "gemm_f16_bias_qgelu_save", "gemm_f32_bias_resid_stats", "gemm_f16_ln_bias",
                                        "gemm_f16_ln_bias_qgelu"};
   ProfScope prof(kNames[EPI], stream);
-  // fp16-output problems go to the 128 x 256 kernel (gemm_wide.cu), other K-major ones to the ping-pong kernel
+  // fp16-output and residual problems go to the 128 x 256 kernel (gemm_wide.cuh), other K-major ones to the ping-pong kernel
   // (gemm_pingpong.cu); both sum the same products in the same order as gemm_f16_kernel, so the same bits.  MN-major
   // operands (pg_gemm_tn) stay on gemm_f16_kernel.
   if (wide) {
-    CUtensorMap tout;   // fp16 [M, N] with row pitch ldo, stored in 64 x 64 boxes
-    if (make_tmap_f16_2d(&tout, p.out, p.M, p.N, p.ldo, 64, 64)) return 1;
-    return gemm_wide_launch(EPI, p.operand_bf16 != 0, ta, tb, tout, a, grid, stream);
+    // [M, N] with row pitch ldo: fp16 in 64 x 64 boxes, fp32 in 64 x 32 boxes (128-byte rows)
+    CUtensorMap tout, tres, taux;
+    if (EpiTraits<EPI>::kResid) {
+      if (make_tmap_f32_2d(&tout, p.out, p.M, p.N, p.ldo, 64, 32)) return 1;
+      if (make_tmap_f32_2d(&tres, a.resid, p.M, p.N, p.ldo, 64, 32)) return 1;
+      if (EpiTraits<EPI>::kStats) {
+        if (make_tmap_f16_2d(&taux, p.aux, p.M, p.N, p.ldo, 64, 64)) return 1;
+      } else {
+        taux = tout;
+      }
+    } else {
+      if (make_tmap_f16_2d(&tout, p.out, p.M, p.N, p.ldo, 64, 64)) return 1;
+      tres = taux = tout;
+    }
+    return gemm_wide_launch(EPI, p.operand_bf16 != 0, ta, tb, tout, tres, taux, a, grid, stream);
   }
   if (!p.mn_major && sched != 1) return gemm_pingpong_launch(EPI, p.operand_bf16 != 0, ta, tb, a, grid, stream);
   if (p.mn_major) return p.operand_bf16 ? launch_kernel<EPI, true, true>(ta, tb, a, grid, stream) : launch_kernel<EPI, false, true>(ta, tb, a, grid, stream);

@@ -1,291 +1,18 @@
-// 128 x 256 cooperative wgmma GEMM for sm_90a (K-major operands, fp16 output):  D[M,N] = A[M,K] * W[N,K]^T  (+ epilogue)
-//
-// Runs the fp16-output epilogues that write nothing but the output (gemm_wide_epilogue: qkv and fc1 of the vision tower).
-// The ping-pong kernel (gemm_pingpong.cu) gives each consumer warpgroup its own 128 x 128 tile and issues 2 x 4
-// m64n128k16 per 64-wide K block, so every W tile is read from shared memory twice.  Here the two consumer warpgroups share
-// one 128 x 256 tile: consumer c owns rows [64 c, 64 c + 64) x 256 columns and issues 4 m64n256k16 per K block.  Per MMA
-// FLOP that moves 3/4 of the TMA bytes into shared memory, reads 5/6 of the operand bytes out of it, and fetches 3/4 of
-// the bytes from L2.  Every output element is the same k16 steps in the same order as in the other two kernels, and the
-// epilogue is epilogue_tile's arithmetic per element, so the outputs are the same bits.
-//
-// CTA = 384 threads, 1 CTA / SM, grid = min(#SM, #tiles); the CTA's i-th tile is blockIdx.x + i * gridDim.x, row-major
-// (m_blk = tile / n_blocks) as in the other kernels:
-//   warpgroup 0     TMA producer (one lane, 24 registers): global -> 3-stage ring (A 128 x 64, W 256 x 64, 128B swizzle)
-//   warpgroups 1, 2 consumers (240 registers each): both read every stage, so a stage's empty barrier counts their 8 warps
-//
-// The price is the epilogue overlap that ping-pong buys: both consumers finish a tile together and the tensor cores idle
-// during its epilogue.  The epilogue is kept short: it runs on the accumulator fragment in registers (bias / LayerNorm,
-// quick-GELU, fp16 round to nearest), writes the fp16 values into the consumer's 128B-swizzled staging tile and one lane
-// stores it with cp.async.bulk.tensor (rows past M and columns past N are clipped by the TMA unit), asynchronously, while
-// the producer already fills the ring for the next tile.
-//
-// Shared memory (214 272 bytes of the 232 448 a block may have):
-//   ring     3 x (16 KB A + 32 KB W)                                                     147 456
-//   staging  one per consumer: 64 rows x 256 fp16 columns as four 64 x 64 boxes (8 KB)    2 x 32 768
-//   slack    1024 (1024-byte alignment of the swizzled tiles) + 256 (mbarriers)
-#include "gemm.h"
-#include "gemm_epilogue.cuh"
-#include "gemm_wide.h"
-#include "ptx.cuh"
-#include "tma_host.h"
-
-#include <atomic>
+// 128 x 256 cooperative wgmma GEMM (gemm_wide.cuh): the fp16-output epilogues (qkv and fc1 of the vision tower) are
+// instantiated here; the fp32 residual epilogues (out_proj and fc2) in gemm_wide_resid.cu.
+#include "gemm_wide.cuh"
 
 namespace pg {
 
-namespace {
-
-constexpr int BLOCK_M = 128;
-constexpr int BLOCK_N = kWideBlockN;
-constexpr int BLOCK_K = 64;
-constexpr int kStages = 3;
-constexpr int kNumThreads = 384;
-constexpr int kProducerRegs = 24;
-constexpr int kConsumerRegs = 240;
-static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register budget of one CTA per SM");
-constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
-constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
-constexpr int kStageBytes = kABytes + kBBytes;
-constexpr int kBoxRows = 64, kBoxCols = 64;                // one TMA store: 64 rows x 128 bytes
-constexpr int kBoxBytes = kBoxRows * kBoxCols * 2;
-constexpr int kOutBytes = (BLOCK_N / kBoxCols) * kBoxBytes;  // one consumer's staging tile
-constexpr int kSmemBytes = kStages * kStageBytes + 2 * kOutBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-static_assert(kSmemBytes <= 232448, "shared memory per block on sm_90");
-static_assert(kBoxBytes % 1024 == 0 && kStageBytes % 1024 == 0, "128B-swizzled tiles start on 1024-byte boundaries");
-constexpr int kConsumerBar = 1;   // + c: the 128 threads of consumer c
-
-// Bias / colsum pair.  A coherent load (not ld.global.nc, which ptxas may move above a barrier): the epilogue's named
-// barriers then keep each box's loads with that box, instead of all 64 being in flight at once next to the 128 accumulators.
-__device__ __forceinline__ float2 ldg_f2(const float* p) {
-  float2 v;
-  asm volatile("ld.global.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
-  return v;
-}
-
-// LayerNorm consumer: out = ln_a * acc + ln_b * colsum + bias, with (ln_a, ln_b) of the A row (= output row) from the
-// producer's per-128-column partials, summed as epilogue_tile (gemm_epilogue.cuh) sums them.
-__device__ __forceinline__ void ln_coeffs(const GemmArgs& args, int row, float& ln_a, float& ln_b) {
-  float s1 = 0.f, s2 = 0.f;
-  if (row < args.M) {
-    const float2* st = reinterpret_cast<const float2*>(args.stats) + (long)row * args.stats_slots;
-    for (int k = 0; k < args.stats_slots; ++k) {
-      const float2 p = st[k];
-      s1 += p.x;
-      s2 += p.y;
-    }
-  }
-  const float inv_k = 1.0f / (float)args.K;
-  const float mu = s1 * inv_k;
-  const float var = fmaxf(s2 * inv_k - mu * mu, 0.f);
-  ln_a = rsqrtf(var + args.ln_eps);
-  ln_b = -ln_a * mu;
-}
-
-// One consumer warpgroup's epilogue of its 64 x 256 part of the tile.  Thread (warp w, lane l) holds rows r = 16 w + l / 4
-// and r + 8 (wgmma.cuh fragment layout; ln_a / ln_b [h] belong to row r + 8 h), columns 8 j + 2 (l % 4) + {0, 1} for
-// j < 32.  Per element it does exactly what epilogue_tile (gemm_epilogue.cuh) does, in the same order.
-template <int EPI>
-__device__ __forceinline__ void wide_epilogue(const GemmArgs& args, const float (&acc)[BLOCK_N / 2], const float (&ln_a)[2],
-                                              const float (&ln_b)[2], const uint8_t* out_tile, const CUtensorMap* tmap_out,
-                                              int c, int warp_in_group, int lane, int tile_row0, int tile_col0) {
-  constexpr bool kLn = EpiTraits<EPI>::kLn;
-  constexpr bool kGelu = (EPI == EPI_F16_BIAS_QGELU || EPI == EPI_F16_LN_BIAS_QGELU);
-  const int rbase = 16 * warp_in_group + (lane >> 2);   // this lane's first row within the consumer's 64
-  const bool tile_in_n = tile_col0 + BLOCK_N <= args.N;
-  const bool store_lane = (warp_in_group | lane) == 0;
-  if (store_lane) bulk_wait_group_read<0>();   // the previous tile's stores have read the staging tile
-  named_barrier_sync(kConsumerBar + c, 128);
-  // 16-byte piece q of staging row r sits at piece slot q ^ (r & 7) (the TMA unit's 128-byte swizzle); rows r and r + 8
-  // share r & 7, and the 8 rows of one store instruction hit 8 different slots: no bank conflicts.
-  const uint32_t srow = smem_u32(out_tile) + (uint32_t)rbase * 128 + (uint32_t)(lane & 3) * 4;
-  const int sw = rbase & 7;
-#pragma unroll
-  for (int j = 0; j < BLOCK_N / 8; ++j) {
-    const int col = tile_col0 + 8 * j + 2 * (lane & 3);
-    float2 b = make_float2(0.f, 0.f), cs = make_float2(0.f, 0.f);
-    if (kLn) {   // N % 64 == 0 (checked at launch): a column pair is wholly inside or past N
-      if (col < args.N) {
-        cs = ldg_f2(args.colsum + col);
-        b = ldg_f2(args.bias + col);
-      }
-    } else if (args.bias != nullptr) {
-      if (tile_in_n) {
-        b = ldg_f2(args.bias + col);
-      } else {
-        if (col < args.N) b.x = __ldg(args.bias + col);
-        if (col + 1 < args.N) b.y = __ldg(args.bias + col + 1);
-      }
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-      if (kLn) {
-        v0 = fmaf(ln_a[h], v0, fmaf(ln_b[h], cs.x, b.x));
-        v1 = fmaf(ln_a[h], v1, fmaf(ln_b[h], cs.y, b.y));
-      } else if (args.bias != nullptr) {
-        v0 += b.x;
-        v1 += b.y;
-      }
-      if (kGelu) {
-        v0 = quick_gelu(v0);
-        v1 = quick_gelu(v1);
-      }
-      sts_u1(srow + (uint32_t)(j >> 3) * kBoxBytes + (uint32_t)(8 * h) * 128 + (uint32_t)(((j & 7) ^ sw) << 4), pack_half2(v0, v1));
-    }
-    // one box at a time: without the barrier ptxas starts every box's loads and MUFU work at once and spills
-    if ((j & 7) == 7 && j + 1 < BLOCK_N / 8) named_barrier_sync(kConsumerBar + c, 128);
-  }
-  fence_proxy_async_smem();   // the generic-proxy writes above, before the TMA unit reads them
-  named_barrier_sync(kConsumerBar + c, 128);
-  if (store_lane && tile_row0 + 64 * c < args.M) {
-#pragma unroll
-    for (int q = 0; q < BLOCK_N / kBoxCols; ++q)
-      if (tile_col0 + q * kBoxCols < args.N)
-        tma_store_2d(tmap_out, out_tile + q * kBoxBytes, tile_col0 + q * kBoxCols, tile_row0 + 64 * c);
-    bulk_commit_group();
-  }
-}
-
-template <int EPI, bool BF16>
-__global__ void __launch_bounds__(kNumThreads, 1)
-gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const __grid_constant__ CUtensorMap tmap_out, const GemmArgs args) {
-  extern __shared__ uint8_t smem_raw[];
-  // 128B-swizzled tiles need 1024-byte alignment.
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * kABytes;
-  uint8_t* smem_out = smem + kStages * kStageBytes;   // the consumers' staging tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_out + 2 * kOutBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + kStages;
-
-  const int wg = threadIdx.x >> 7;
-  const int warp_in_group = (threadIdx.x >> 5) & 3;
-  const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_out);
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);  // one arrive per warp of both consumers
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (wg == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec<kProducerRegs>();
-    // (the tile counts are computed after setmaxnreg by each role: a value live across it is spilled)
-    const int n_blocks = (args.N + BLOCK_N - 1) / BLOCK_N;
-    const int num_tiles = (args.M + BLOCK_M - 1) / BLOCK_M * n_blocks;
-    const int num_kb = (args.K + BLOCK_K - 1) / BLOCK_K;
-    if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_2d(smem_a + stage * kABytes, &tmap_a, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
-          tma_load_2d(smem_b + stage * kBBytes, &tmap_b, &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    return;
-  }
-
-  // -------------------------------------------------------------------- consumer warpgroups
-  setmaxnreg_inc<kConsumerRegs>();
-  const int n_blocks = (args.N + BLOCK_N - 1) / BLOCK_N;
-  const int num_tiles = (args.M + BLOCK_M - 1) / BLOCK_M * n_blocks;
-  const int num_kb = (args.K + BLOCK_K - 1) / BLOCK_K;
-  const int c = wg - 1;
-  const uint8_t* out_tile = smem_out + c * kOutBytes;
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
-    // LayerNorm coefficients of this lane's two rows, before the accumulators are live (with them live the epilogue spills)
-    float ln_a[2] = {1.f, 1.f}, ln_b[2] = {0.f, 0.f};
-    if (EpiTraits<EPI>::kLn) {
-      const int row0 = m_blk * BLOCK_M + 64 * c + 16 * warp_in_group + (lane >> 2);
-      ln_coeffs(args, row0, ln_a[0], ln_b[0]);
-      ln_coeffs(args, row0 + 8, ln_a[1], ln_b[1]);
-    }
-    // The first MMA of the tile overwrites the accumulators (scale-d 0); defining them here ends their live range at the
-    // previous tile's epilogue.
-    float acc[BLOCK_N / 2];
-#pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-    int prev_stage = -1;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t a_addr = smem_u32(smem_a + stage * kABytes + c * (kABytes / 2));   // rows [64 c, 64 c + 64) of the tile
-      const uint32_t b_addr = smem_u32(smem_b + stage * kBBytes);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BLOCK_K / 16; ++k) {
-        const uint64_t a_desc = make_smem_desc(a_addr + k * 32, 16, 1024);
-        const uint64_t b_desc = make_smem_desc(b_addr + k * 32, 16, 1024);
-        if (BF16) wgmma_ss_n256_bf16<0, 0>(acc, a_desc, b_desc, (kb | k) != 0);
-        else      wgmma_ss_n256_f16<0, 0>(acc, a_desc, b_desc, (kb | k) != 0);
-      }
-      wgmma_commit();
-      if (prev_stage >= 0) {   // the previous K block's MMAs have retired: this warp is done with its smem slot
-        wgmma_wait<1>();
-        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      }
-      prev_stage = stage;
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-
-    wide_epilogue<EPI>(args, acc, ln_a, ln_b, out_tile, &tmap_out, c, warp_in_group, lane, m_blk * BLOCK_M, n_blk * BLOCK_N);
-  }
-  if ((warp_in_group | lane) == 0) bulk_wait_group<0>();   // the last tile's stores are complete before the CTA exits
-}
-
-template <int EPI, bool BF16>
-int launch_kernel(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const GemmArgs& a, int grid,
-                  cudaStream_t stream) {
-  auto kern = gemm_wide_kernel<EPI, BF16>;
-  static std::atomic<int> attr_set[64];   // per template instantiation and device (the attribute is per context)
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  if (!attr_set[dev].load(std::memory_order_acquire)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) { set_last_error("gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return 1; }
-    attr_set[dev].store(1, std::memory_order_release);
-  }
-  kern<<<grid, kNumThreads, kSmemBytes, stream>>>(ta, tb, tout, a);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error("gemm launch: %s", cudaGetErrorString(e)); return 1; }
-  return 0;
-}
-
-template <int EPI>
-int launch(bool bf16, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const GemmArgs& a, int grid,
-           cudaStream_t stream) {
-  return bf16 ? launch_kernel<EPI, true>(ta, tb, tout, a, grid, stream) : launch_kernel<EPI, false>(ta, tb, tout, a, grid, stream);
-}
-
-}  // namespace
-
 int gemm_wide_launch(int epi, bool bf16, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
-                     const GemmArgs& a, int grid, cudaStream_t stream) {
+                     const CUtensorMap& tres, const CUtensorMap& taux, const GemmArgs& a, int grid, cudaStream_t stream) {
   switch (epi) {
-    case EPI_F16_BIAS:           return launch<EPI_F16_BIAS>(bf16, ta, tb, tout, a, grid, stream);
-    case EPI_F16_BIAS_QGELU:     return launch<EPI_F16_BIAS_QGELU>(bf16, ta, tb, tout, a, grid, stream);
-    case EPI_F16_LN_BIAS:        return launch<EPI_F16_LN_BIAS>(bf16, ta, tb, tout, a, grid, stream);
-    case EPI_F16_LN_BIAS_QGELU:  return launch<EPI_F16_LN_BIAS_QGELU>(bf16, ta, tb, tout, a, grid, stream);
+    case EPI_F16_BIAS:              return launch<EPI_F16_BIAS>(bf16, ta, tb, tout, tres, taux, a, grid, stream);
+    case EPI_F16_BIAS_QGELU:        return launch<EPI_F16_BIAS_QGELU>(bf16, ta, tb, tout, tres, taux, a, grid, stream);
+    case EPI_F16_LN_BIAS:           return launch<EPI_F16_LN_BIAS>(bf16, ta, tb, tout, tres, taux, a, grid, stream);
+    case EPI_F16_LN_BIAS_QGELU:     return launch<EPI_F16_LN_BIAS_QGELU>(bf16, ta, tb, tout, tres, taux, a, grid, stream);
+    case EPI_F32_BIAS_RESID:
+    case EPI_F32_BIAS_RESID_STATS:  return gemm_wide_resid_launch(epi, bf16, ta, tb, tout, tres, taux, a, grid, stream);
     default: set_last_error("gemm: epilogue %d has no 128 x 256 kernel", epi); return 1;
   }
 }

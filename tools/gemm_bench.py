@@ -1,13 +1,14 @@
 """GEMM schedules on one GPU: the automatic choice (schedule 0, the default: the 128 x 256 kernel for the fp16-output
-projections, ping-pong for the rest) against the ping-pong kernel for every K-major GEMM (schedule 2,
-pg_gemm_set_schedule).  Writes one JSON file, <out>/gemm_bench.json, with the card's name, power limit and SM clocks
+projections and the fp32 residual updates, ping-pong for the rest) against the ping-pong kernel for every K-major GEMM
+(schedule 2, pg_gemm_set_schedule).  Writes one JSON file, <out>/gemm_bench.json, with the card's name, power limit and SM clocks
 (read-only nvidia-smi queries) beside the numbers.
 
   1. per GEMM family at the real shapes: VitEngine.forward on --views views of ViT-L/14-336 (LayerNorm folded), device
      time per family from the library's launch events, both schedules alternating, --rounds rounds each;
   2. K-sweep: M = 590 848 (1024 views x 577 tokens), N in {1024, 3072}, K in {256 .. 4096}, EPI_F16_BIAS and
-     EPI_F16_BIAS_QGELU, both schedules, fitted to t = a + b K: b gives the mainloop rate, a the per-tile fixed cost
-     (epilogue, fill, drain); torch.matmul (cuBLAS) at the same shapes as a reference point on the same card;
+     EPI_F16_BIAS_QGELU, and at N = 1024 EPI_F32_BIAS_RESID_STATS in place (K = 1024 is out_proj, K = 4096 fc2, which
+     the per-family profile cannot tell apart), both schedules, fitted to t = a + b K: b gives the mainloop rate, a the
+     per-tile fixed cost (epilogue, fill, drain); torch.matmul (cuBLAS) at the same shapes as a reference point on the same card;
   3. --bench-ab: bench.py --steps 10 --warmup 3 --no-cpu-baseline --dump-outputs as a subprocess, 3 times with
      PG_GEMM_SCHEDULE=2 and 3 times without, alternating; every dumped array of the two schedules compared bit for bit.
 
@@ -124,12 +125,26 @@ def sweep(reps=5):
     for N in (1024, 3072):
         w = (torch.randn(N, Kmax, device="cuda", generator=g) * 0.03).half()
         bias = torch.randn(N, device="cuda", generator=g)
-        for epi, name in ((0, "EPI_F16_BIAS"), (1, "EPI_F16_BIAS_QGELU")):
-            o = torch.empty(M, N, device="cuda", dtype=torch.float16)
+        epis = ((0, "EPI_F16_BIAS"), (1, "EPI_F16_BIAS_QGELU")) + (((7, "EPI_F32_BIAS_RESID_STATS"),) if N == 1024 else ())
+        for epi, name in epis:
+            if epi == 7:   # the residual stream updated in place, its fp16 copy and per-128-column moments (out_proj, fc2)
+                o = torch.randn(M, N, device="cuda", generator=g)
+                aux = torch.empty(M, N, device="cuda", dtype=torch.float16)
+                stats = torch.empty(M, N // 128, 2, device="cuda")
+
+                def run(K):
+                    p = _lib.GemmProblem(M=M, N=N, K=K, a=ptr(a), lda=Kmax, w=ptr(w), ldw=Kmax, out=ptr(o), ldo=N, bias=ptr(bias),
+                                         epilogue=epi, aux=ptr(aux), stats=ptr(stats))
+                    check(lib.pg_gemm_problem_run(C.byref(p), current_stream_ptr()), "pg_gemm_problem_run")
+            else:
+                o = torch.empty(M, N, device="cuda", dtype=torch.float16)
+
+                def run(K):
+                    check(lib.pg_gemm_f16(ptr(a), Kmax, ptr(w), Kmax, ptr(o), N, ptr(bias), M, N, K, epi, current_stream_ptr()),
+                          "pg_gemm_f16")
             for sched in SCHEDULES:
                 ops.gemm_set_schedule(sched)
-                ts = [timed(lambda: check(lib.pg_gemm_f16(ptr(a), Kmax, ptr(w), Kmax, ptr(o), N, ptr(bias), M, N, K, epi,
-                                                          current_stream_ptr()), "pg_gemm_f16")) for K in SWEEP_K]
+                ts = [timed(lambda: run(K)) for K in SWEEP_K]
                 b, a0 = np.polyfit(np.array(SWEEP_K, dtype=float), np.array(ts), 1)
                 tiles = (M // 128) * (N // (256 if sched == 0 else 128))
                 out["configs"][f"N{N}_{name}_schedule{sched}"] = {
@@ -138,6 +153,8 @@ def sweep(reps=5):
                     "mainloop_tflops_from_slope": 2 * M * N / (b / 1e3) / 1e12,
                     "fixed_us_per_tile_per_sm": a0 * 1e3 / (tiles / torch.cuda.get_device_properties(0).multi_processor_count)}
             del o
+            if epi == 7:
+                del aux, stats
         ops.gemm_set_schedule(0)
         ts = []
         for K in SWEEP_K:
