@@ -202,7 +202,8 @@ int pg_preprocess_clip(const pg_image* images, int32_t n, int32_t size, const fl
  * finetune_dataset.py:86-90), dataset_creation/benchmark/benchmark_dataset.py:66-79 and pretrain_dataset.py:109-161.
  * Byte-identical to Pillow over libjpeg-turbo with its defaults (ISLOW IDCT, fancy upsampling) for the files it
  * decodes: sequential Huffman (SOF0 / SOF1), 8-bit, one scan, grayscale or YCbCr 4:4:4 / 4:2:2 / 4:2:0, with or
- * without restart markers.  Everything else is refused with a status and a reason (DESIGN.md §1).
+ * without restart markers; through pg_jpeg_parse_multiscan also progressive (SOF2) and multi-scan sequential files of
+ * the same kinds.  Everything else is refused with a status and a reason (DESIGN.md §1).
  * ------------------------------------------------------------------------------------------------- */
 #define PG_JPEG_OK 0
 #define PG_JPEG_UNSUPPORTED 1       /* a valid file outside the decoded subset: progressive, 12-bit, CMYK, RGB, ... */
@@ -220,7 +221,8 @@ typedef struct pg_jpeg_info {
   int32_t component_id[3], h_samp[3], v_samp[3], quant_table[3], dc_table[3], ac_table[3];
   int32_t restart_interval;       /* MCUs per restart interval, 0 without DRI */
   int32_t num_segments;           /* entropy-coded segments: restart intervals, or 1 */
-  int32_t table_mask;             /* bit t: DQT t defined; bit 4 + t: DC DHT t; bit 8 + t: AC DHT t */
+  int32_t table_mask;             /* bit t: DQT t defined; bit 4 + t: DC DHT t; bit 8 + t: AC DHT t;
+                                     PG_JPEG_MULTISCAN and bits 16+ for multi-scan files (below) */
   int64_t scan_offset, scan_bytes; /* entropy-coded data, from the end of the SOS segment to the marker after it */
   uint16_t qt[4][64];             /* quantisation tables in zig-zag order, as stored */
   uint8_t dc_bits[4][16], ac_bits[4][16];
@@ -230,13 +232,41 @@ typedef struct pg_jpeg_info {
 /* Host-only marker walk of one file (data_host: `bytes` bytes).  Returns info_out->status; when it is not PG_JPEG_OK,
  * pg_last_error() names the reason.  Validates the restart-marker sequence and the EOI. */
 int pg_jpeg_parse(const uint8_t* data_host, int64_t bytes, pg_jpeg_info* info_out);
+
+/* Multi-scan files: progressive Huffman (SOF2, 8-bit) and sequential SOF0 / SOF1 files of more than one scan, with the
+ * components and sampling layouts above.  pg_jpeg_parse_multiscan returns, for every file pg_jpeg_parse accepts, the
+ * identical info; it also accepts these files, marking them with PG_JPEG_MULTISCAN in table_mask.  For such an info:
+ * num_segments counts the entropy-coded segments of all scans, scan_offset / scan_bytes span the data from the first
+ * scan to the EOI, restart_interval is that of the first scan, and table_mask >> 16 is the number of Huffman table
+ * selections over all scans (it bounds the workspace).  The per-scan tables are found again from the file's bytes by
+ * pg_jpeg_decode.  libjpeg's JERR_BAD_PROGRESSION cases are PG_JPEG_BAD_HEADER; sequences libjpeg only warns about
+ * (JWRN_BOGUS_PROGRESSION), a coefficient sent twice, more than PG_JPEG_MAX_SCANS scans and a progression that leaves
+ * any coefficient unsent or not refined to bit 0 (libjpeg then smooths between blocks) are PG_JPEG_UNSUPPORTED. */
+#define PG_JPEG_MULTISCAN (1 << 12)
+#define PG_JPEG_MAX_SCANS 256
+int pg_jpeg_parse_multiscan(const uint8_t* data_host, int64_t bytes, pg_jpeg_info* info_out);
+
+typedef struct pg_jpeg_scan {
+  int32_t components;             /* in this scan: 1, or the interleaved components of a sequential or DC scan */
+  int32_t component[3];           /* frame component indices (0 .. components of the frame - 1), in scan order */
+  int32_t ss, se, ah, al;         /* spectral band and successive-approximation bits (0, 63, 0, 0 when sequential) */
+  int32_t restart_interval;       /* MCUs per restart interval (single blocks in a one-component scan), 0 without DRI */
+  int32_t num_segments;           /* entropy-coded segments of this scan */
+  int32_t level;                  /* 1 + the highest level of earlier scans sharing a component and a coefficient */
+} pg_jpeg_scan;
+/* Host-only: the scans of a file pg_jpeg_parse_multiscan accepts (one for a single-scan file), the first min(count,
+ * cap) written to out.  Returns their count, or -1 (pg_last_error() names the reason) for a refused file. */
+int pg_jpeg_scans(const uint8_t* data_host, int64_t bytes, pg_jpeg_scan* out, int32_t cap);
+
 /* Workspace of pg_jpeg_decode for n parsed files packed into packed_bytes bytes.  0 on error. */
 size_t pg_jpeg_workspace_bytes(const pg_jpeg_info* infos_host, int32_t n, int64_t packed_bytes);
 /* Decodes the files whose info status is PG_JPEG_OK: file i is packed_host[offsets_host[i] .. offsets_host[i+1]) (one
  * host-to-device copy of offsets_host[n] bytes; pinned memory makes it asynchronous), infos_host[i] its pg_jpeg_parse
- * result, dst_host[i] a descriptor of its height x width x 3 uint8 RGB destination (written; the same descriptors feed
- * pg_preprocess_clip).  status_out: device i32 [n], the parse status of a skipped file, else PG_JPEG_OK or the
- * entropy-data error of that file (whose destination is then left unwritten).  Three launches for the whole batch. */
+ * or pg_jpeg_parse_multiscan result, dst_host[i] a descriptor of its height x width x 3 uint8 RGB destination
+ * (written; the same descriptors feed pg_preprocess_clip).  status_out: device i32 [n], the parse status of a skipped
+ * file, else PG_JPEG_OK or the entropy-data error of that file (whose destination is then left unwritten).  Three
+ * launches for a batch of single-scan files.  A batch with multi-scan files also zeroes their coefficients and decodes
+ * their scans in one launch per dependency level (pg_jpeg_scan.level), all in stream order. */
 int pg_jpeg_decode(const uint8_t* packed_host, const int64_t* offsets_host, const pg_jpeg_info* infos_host, int32_t n,
                    const pg_image* dst_host, void* workspace, size_t workspace_bytes, int32_t* status_out, void* stream);
 

@@ -99,6 +99,11 @@ class JpegInfo(C.Structure):
                 ("ac_vals", (C.c_uint8 * 256) * 4)]
 
 
+class JpegScan(C.Structure):
+    _fields_ = [("components", c_int32), ("component", c_int32 * 3), ("ss", c_int32), ("se", c_int32), ("ah", c_int32),
+                ("al", c_int32), ("restart_interval", c_int32), ("num_segments", c_int32), ("level", c_int32)]
+
+
 class GemmProblem(C.Structure):
     _fields_ = [("M", c_int32), ("N", c_int32), ("K", c_int32), ("a", c_void_p), ("lda", c_int32), ("w", c_void_p),
                 ("ldw", c_int32), ("out", c_void_p), ("ldo", c_int32), ("bias", c_void_p), ("epilogue", c_int32),
@@ -171,6 +176,8 @@ SIGNATURES = {
     "pg_preprocess_clip": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int32,
                                      c_void_p]),
     "pg_jpeg_parse": (c_int32, [c_void_p, c_int64, C.POINTER(JpegInfo)]),
+    "pg_jpeg_parse_multiscan": (c_int32, [c_void_p, c_int64, C.POINTER(JpegInfo)]),
+    "pg_jpeg_scans": (c_int32, [c_void_p, c_int64, C.POINTER(JpegScan), c_int32]),
     "pg_jpeg_workspace_bytes": (c_size_t, [C.POINTER(JpegInfo), c_int32, c_int64]),
     "pg_jpeg_decode": (c_int32, [c_void_p, c_void_p, C.POINTER(JpegInfo), c_int32, c_void_p, c_void_p, c_size_t, c_void_p,
                                  c_void_p]),

@@ -7,6 +7,10 @@
 //             post-IDCT range-limit table with its `& RANGE_MASK` wrap -> component planes padded to whole MCUs;
 //   kernel 3  fancy upsampling (jdsample.c h2v1 / h2v2, plain replication when the chroma width is <= 2) fused with
 //             jdcolor.c's fixed-point YCbCr->RGB (SCALEBITS 16) -> uint8 RGB rows in the caller's pg_image destinations.
+// Multi-scan files (progressive SOF2, or sequential in several scans; pg_jpeg_parse_multiscan) differ only in how the
+// coefficients are filled: their blocks are zeroed, then multiscan_kernel decodes one thread per segment of every scan
+// (DC / AC first and refinement scans with jdphuff.c's arithmetic), one launch per dependency level: a scan runs after
+// every earlier scan that shares a component and a coefficient with it.  Kernels 2 and 3 are the same for both.
 // Per-image status: a corrupt image stops its own segments and is not colour-converted; the other images are unaffected.
 // Every read is bounded by the image's own segment, every write by its own planes and destination.
 #include <cuda_runtime.h>
@@ -169,20 +173,61 @@ int walk_scan(const uint8_t* d, int64_t n, int64_t pos, std::vector<std::pair<in
   }
 }
 
-int parse(const uint8_t* d, int64_t n, pg_jpeg_info* info, std::vector<std::pair<int64_t, int64_t>>* segs, Why* why) {
+// One scan of a multi-scan file, as the multi-scan walk finds it: what pg_jpeg_scans reports, plus the Huffman tables
+// the scan selected (copied at its SOS: a later DHT may redefine them) and, when asked for, its segments.
+struct ScanRec {
+  pg_jpeg_scan pub;
+  uint8_t dc_bits[3][16], ac_bits[3][16];
+  uint8_t dc_vals[3][256], ac_vals[3][256];
+  std::vector<std::pair<int64_t, int64_t>> segs;
+};
+
+struct MultiScan {
+  bool want_segs = false;
+  bool multi = false;                // progressive, more than one scan, or one scan that is not all components in order
+  std::vector<ScanRec> scans;
+  uint16_t qt[3][64];                // quantisation table of each component, latched at its first scan (zig-zag)
+  bool latched[3] = {false, false, false};
+  int coef_bits[3][64];              // jdphuff.c coef_bits: bit position each coefficient has reached, -1 before any
+  int tables = 0;                    // Huffman table selections over all scans
+  int64_t first_scan = 0, eoi = 0;
+};
+
+int parse_scan(const uint8_t* d, int64_t n, const uint8_t* s, int len, int64_t pos, pg_jpeg_info* info, MultiScan* ms,
+               bool saw_jfif, bool saw_adobe, int adobe_transform, int64_t* next, Why* why);
+int finish_multiscan(pg_jpeg_info* info, MultiScan* ms, Why* why);
+
+// The marker walk of pg_jpeg_parse; with `ms` that of pg_jpeg_parse_multiscan, which also takes SOF2 and any number
+// of scans, and lets DHT / DQT / DRI / APPn / COM appear between scans.
+int parse(const uint8_t* d, int64_t n, pg_jpeg_info* info, std::vector<std::pair<int64_t, int64_t>>* segs, Why* why,
+          MultiScan* ms = nullptr) {
   memset(info, 0, sizeof(*info));
   if (!d || n < 4 || d[0] != 0xFF || d[1] != 0xD8) return info->status = why->set(PG_JPEG_BAD_HEADER, "no SOI marker");
   int64_t pos = 2;
   bool saw_jfif = false, saw_adobe = false, saw_sof = false;
   int adobe_transform = -1;
   for (;;) {
+    const bool after_scan = ms && !ms->scans.empty();
+    if (pos >= n && after_scan) return info->status = why->set(PG_JPEG_NO_EOI, "no EOI after the last scan");
     if (pos >= n) return info->status = why->set(PG_JPEG_BAD_HEADER, "truncated before the scan");
     if (d[pos] != 0xFF)
       return info->status = why->set(PG_JPEG_BAD_HEADER, "expected a marker at byte %lld", (long long)pos);
+    const int64_t marker_pos = pos;
     while (pos < n && d[pos] == 0xFF) ++pos;            // fill bytes before a marker
+    if (pos >= n && after_scan) return info->status = why->set(PG_JPEG_NO_EOI, "no EOI after the last scan");
     if (pos >= n) return info->status = why->set(PG_JPEG_BAD_HEADER, "truncated before the scan");
     const int m = d[pos++];
     if (m == 0x01) continue;                            // TEM: standalone, ignored as libjpeg does
+    if (after_scan) {
+      if (m == 0xD9) {
+        ms->eoi = marker_pos;
+        return info->status = finish_multiscan(info, ms, why);
+      }
+      if ((m >= 0xD0 && m <= 0xD7) || m == 0x00 || m == 0xD8)
+        return info->status = why->set(PG_JPEG_UNEXPECTED_MARKER, "marker 0x%02X between scans", m);
+      if (pos + 2 > n || be16(d + pos) < 2 || pos + be16(d + pos) > n)
+        return info->status = why->set(PG_JPEG_NO_EOI, "truncated between scans");
+    }
     if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x00)
       return info->status = why->set(PG_JPEG_BAD_HEADER, "marker 0x%02X before the first scan", m);
     if (pos + 2 > n) return info->status = why->set(PG_JPEG_BAD_HEADER, "truncated marker 0x%02X", m);
@@ -200,7 +245,8 @@ int parse(const uint8_t* d, int64_t n, pg_jpeg_info* info, std::vector<std::pair
       info->height = be16(s + 1);
       info->width = be16(s + 3);
       info->components = s[5];
-      if (m != 0xC0 && m != 0xC1) {
+      if (ms && m == 0xC2) ms->multi = true;
+      if (m != 0xC0 && m != 0xC1 && !(ms && m == 0xC2)) {
         const char* kind = m == 0xC2 || m == 0xC6 || m == 0xCA || m == 0xCE ? "progressive"
                            : m == 0xC3 || m == 0xC7 || m == 0xCB || m == 0xCF ? "lossless"
                                                                                : "hierarchical or arithmetic";
@@ -280,6 +326,11 @@ int parse(const uint8_t* d, int64_t n, pg_jpeg_info* info, std::vector<std::pair
         return info->status = why->set(PG_JPEG_UNSUPPORTED, "height defined by DNL is not decoded");
       case 0xDA: {                                      // SOS
         if (!saw_sof) return info->status = why->set(PG_JPEG_BAD_HEADER, "scan before the frame header");
+        if (ms) {
+          const int st = parse_scan(d, n, s, len, pos, info, ms, saw_jfif, saw_adobe, adobe_transform, &pos, why);
+          if (st) return info->status = st;
+          break;
+        }
         const int ns = len >= 1 ? s[0] : 0;
         if (len != 4 + 2 * ns || ns < 1) return info->status = why->set(PG_JPEG_BAD_HEADER, "bad SOS segment");
         if (ns != info->components)
@@ -343,6 +394,170 @@ int parse(const uint8_t* d, int64_t n, pg_jpeg_info* info, std::vector<std::pair
         return info->status = why->set(PG_JPEG_BAD_HEADER, "unknown marker 0x%02X", m);
     }
   }
+}
+
+// Blocks per row and rows of the scan's MCU grid: the frame's MCUs when interleaved, else the single component's own
+// blocks, ceil(downsampled size / 8) per side (jdinput.c per_scan_setup).
+void scan_grid(const pg_jpeg_info* info, int ncomp_scan, int c, int* cols, int* rows) {
+  const int hmax = info->components == 3 ? info->h_samp[0] : 1, vmax = info->components == 3 ? info->v_samp[0] : 1;
+  if (ncomp_scan > 1) {
+    *cols = (info->width + 8 * hmax - 1) / (8 * hmax);
+    *rows = (info->height + 8 * vmax - 1) / (8 * vmax);
+    return;
+  }
+  const int h = info->components == 3 ? info->h_samp[c] : 1, v = info->components == 3 ? info->v_samp[c] : 1;
+  *cols = (int)(((long long)info->width * h + 8LL * hmax - 1) / (8LL * hmax));
+  *rows = (int)(((long long)info->height * v + 8LL * vmax - 1) / (8LL * vmax));
+}
+
+// One SOS of the multi-scan walk (s: its segment, pos: the first entropy-coded byte).  Validates the scan as libjpeg
+// 3.1 does at the start of its pass (jdphuff.c start_pass_phuff_decoder, jdhuff.c start_pass_huff_decoder, jdinput.c
+// latch_quant_tables), walks its entropy-coded data and sets *next to the marker that ends it.
+int parse_scan(const uint8_t* d, int64_t n, const uint8_t* s, int len, int64_t pos, pg_jpeg_info* info, MultiScan* ms,
+               bool saw_jfif, bool saw_adobe, int adobe_transform, int64_t* next, Why* why) {
+  const bool progressive = info->sof == 0xC2;
+  const int ns = len >= 1 ? s[0] : 0;
+  if (len != 4 + 2 * ns || ns < 1 || ns > info->components) return why->set(PG_JPEG_BAD_HEADER, "bad SOS segment");
+  if ((int)ms->scans.size() >= PG_JPEG_MAX_SCANS)
+    return why->set(PG_JPEG_UNSUPPORTED, "more than %d scans", PG_JPEG_MAX_SCANS);
+  ms->scans.emplace_back();
+  ScanRec& sc = ms->scans.back();
+  memset(&sc.pub, 0, sizeof(sc.pub));
+  pg_jpeg_scan& p = sc.pub;
+  p.components = ns;
+  const uint8_t* t = s + 1 + 2 * ns;
+  p.ss = t[0];
+  p.se = t[1];
+  p.ah = t[2] >> 4;
+  p.al = t[2] & 15;
+  if (ns != info->components || ms->scans.size() > 1) ms->multi = true;
+  for (int j = 0; j < ns; ++j) {
+    int c = 0;
+    while (c < info->components && info->component_id[c] != s[1 + 2 * j]) ++c;
+    if (c == info->components) return why->set(PG_JPEG_BAD_HEADER, "scan component id %d is not in the frame", s[1 + 2 * j]);
+    for (int i = 0; i < j; ++i)
+      if (p.component[i] == c) return why->set(PG_JPEG_BAD_HEADER, "component id %d twice in one scan", s[1 + 2 * j]);
+    if (c != j) ms->multi = true;
+    p.component[j] = c;
+    info->dc_table[c] = s[2 + 2 * j] >> 4;
+    info->ac_table[c] = s[2 + 2 * j] & 15;
+    if (info->dc_table[c] > 3 || info->ac_table[c] > 3) return why->set(PG_JPEG_BAD_HEADER, "bad Huffman table index");
+  }
+  const bool dc_band = p.ss == 0;
+  if (progressive) {                                    // JERR_BAD_PROGRESSION
+    const bool bad = (dc_band ? p.se != 0 : (p.ss > p.se || p.se > 63 || ns != 1)) ||
+                     (p.ah != 0 && p.al != p.ah - 1) || p.al > 13;
+    if (bad) return why->set(PG_JPEG_BAD_HEADER, "bad progression: Ss=%d Se=%d Ah=%d Al=%d", p.ss, p.se, p.ah, p.al);
+  } else if (p.ss != 0 || p.se != 63 || t[2] != 0) {
+    return why->set(PG_JPEG_BAD_HEADER, "spectral selection %d..%d / approximation %d in a sequential scan", t[0], t[1],
+                    t[2]);
+  }
+  if (ms->scans.size() == 1) {
+    ms->first_scan = pos;
+    if (info->components == 3 && !saw_jfif) {           // as in the single-scan walk
+      const bool rgb = saw_adobe ? adobe_transform == 0
+                                 : (info->component_id[0] == 'R' && info->component_id[1] == 'G' &&
+                                    info->component_id[2] == 'B');
+      if (rgb) return why->set(PG_JPEG_UNSUPPORTED, "RGB colour transform is not decoded");
+    }
+  }
+  const bool need_dc = !progressive || (dc_band && p.ah == 0), need_ac = !progressive || !dc_band;
+  for (int j = 0; j < ns; ++j) {
+    const int c = p.component[j];
+    if (!ms->latched[c]) {
+      if (!(info->table_mask & (1 << info->quant_table[c])))
+        return why->set(PG_JPEG_BAD_HEADER, "component %d uses an undefined table", c);
+      memcpy(ms->qt[c], info->qt[info->quant_table[c]], sizeof(ms->qt[c]));
+      ms->latched[c] = true;
+    }
+    const int td = info->dc_table[c], ta = info->ac_table[c];
+    if ((need_dc && !(info->table_mask & (16 << td))) || (need_ac && !(info->table_mask & (256 << ta))))
+      return why->set(PG_JPEG_BAD_HEADER, "component %d uses an undefined table", c);
+    if ((need_dc && !make_huff(info->dc_bits[td], info->dc_vals[td], true, nullptr)) ||
+        (need_ac && !make_huff(info->ac_bits[ta], info->ac_vals[ta], false, nullptr)))
+      return why->set(PG_JPEG_BAD_HEADER, "invalid Huffman table");
+    memcpy(sc.dc_bits[j], info->dc_bits[td], 16);
+    memcpy(sc.dc_vals[j], info->dc_vals[td], 256);
+    memcpy(sc.ac_bits[j], info->ac_bits[ta], 16);
+    memcpy(sc.ac_vals[j], info->ac_vals[ta], 256);
+    ms->tables += need_dc + need_ac;
+    // progression state (jdphuff.c): what libjpeg only warns about is left to the host decoder
+    if (progressive && !dc_band && ms->coef_bits[c][0] < 0)
+      return why->set(PG_JPEG_UNSUPPORTED, "bogus progression: AC scan of component %d before its DC scan", c);
+    for (int k = p.ss; k <= p.se; ++k) {
+      const int cur = ms->coef_bits[c][k];
+      if (progressive && p.ah != (cur < 0 ? 0 : cur))
+        return why->set(PG_JPEG_UNSUPPORTED, "bogus progression: scan with Ah=%d for coefficient %d of component %d at bit %d",
+                        p.ah, k, c, cur);
+      if (progressive && p.ah == 0 && cur >= 0)
+        return why->set(PG_JPEG_UNSUPPORTED, "coefficient %d of component %d is sent twice", k, c);
+      ms->coef_bits[c][k] = p.al;
+    }
+  }
+  // dependency level: after every earlier scan that shares a component and a coefficient position
+  p.level = 1;
+  for (size_t i = 0; i + 1 < ms->scans.size(); ++i) {
+    const pg_jpeg_scan& q = ms->scans[i].pub;
+    if (q.ss > p.se || p.ss > q.se) continue;
+    bool shared = false;
+    for (int a = 0; a < q.components; ++a)
+      for (int b = 0; b < ns; ++b) shared |= q.component[a] == p.component[b];
+    if (shared) p.level = std::max(p.level, q.level + 1);
+  }
+  p.restart_interval = info->restart_interval;
+  int nseg = 0;
+  int64_t mp = 0;
+  const int st = walk_scan(d, n, pos, ms->want_segs ? &sc.segs : nullptr, &nseg, &mp, why);
+  if (st) return st;
+  int cols = 0, rows = 0;
+  scan_grid(info, ns, p.component[0], &cols, &rows);
+  const long long mcus = (long long)cols * rows;
+  const long long want = p.restart_interval ? (mcus + p.restart_interval - 1) / p.restart_interval : 1;
+  if (nseg != want)
+    return why->set(PG_JPEG_BAD_RST, "scan %d: %d entropy-coded segments where %lld were expected",
+                    (int)ms->scans.size(), nseg, want);
+  p.num_segments = nseg;
+  *next = mp;
+  return PG_JPEG_OK;
+}
+
+// At the EOI of a multi-scan file: every coefficient of every component sent and refined to bit 0 (else libjpeg would
+// smooth the blocks of a progressive file, or leave a component blank), then the info fields of a multi-scan file.
+int finish_multiscan(pg_jpeg_info* info, MultiScan* ms, Why* why) {
+  for (int c = 0; c < info->components; ++c)
+    for (int k = 0; k < 64; ++k)
+      if (ms->coef_bits[c][k] != 0) {
+        if (info->sof != 0xC2) return why->set(PG_JPEG_UNSUPPORTED, "component %d has no scan", c);
+        return why->set(PG_JPEG_UNSUPPORTED, "incomplete progression: coefficient %d of component %d %s", k, c,
+                        ms->coef_bits[c][k] < 0 ? "is never sent" : "is not refined to bit 0");
+      }
+  long long segs = 0;
+  for (const ScanRec& sc : ms->scans) segs += sc.pub.num_segments;
+  if (segs > 0x7fffffff) return why->set(PG_JPEG_UNSUPPORTED, "too many entropy-coded segments");
+  info->num_segments = (int32_t)segs;
+  info->restart_interval = ms->scans[0].pub.restart_interval;
+  info->scan_offset = ms->first_scan;
+  info->scan_bytes = ms->eoi - ms->first_scan;
+  info->table_mask = (info->table_mask & 0xFFF) | PG_JPEG_MULTISCAN | (ms->tables << 16);
+  return PG_JPEG_OK;
+}
+
+// pg_jpeg_parse_multiscan: the single-scan walk's result for every file that is not multi-scan (so that a file
+// pg_jpeg_parse accepts gets the identical info), else the multi-scan walk's.
+int parse_multiscan(const uint8_t* d, int64_t n, pg_jpeg_info* info, MultiScan* ms, Why* why) {
+  const int st = parse(d, n, info, nullptr, why);
+  if (st == PG_JPEG_OK) return st;
+  std::vector<char> msg2(why->len);
+  Why why2{msg2.data(), msg2.size()};
+  msg2[0] = 0;
+  pg_jpeg_info mi;
+  for (int c = 0; c < 3; ++c)
+    for (int k = 0; k < 64; ++k) ms->coef_bits[c][k] = -1;
+  const int st2 = parse(d, n, &mi, nullptr, &why2, ms);
+  if (!ms->multi) return st;
+  *info = mi;
+  snprintf(why->buf, why->len, "%s", msg2.data());
+  return st2;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -477,6 +692,153 @@ entropy_kernel(const uint8_t* __restrict__ bytes, const ImgDesc* __restrict__ im
   const Seg sg = segs[si];
   const ImgDesc& im = imgs[sg.img];
   const int err = decode_segment(bytes, im, tbls, sg, blk_smem[lane], coef);
+  if (err) atomicCAS(status + im.orig, 0, err);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Device: entropy decode of multi-scan files
+// ------------------------------------------------------------------------------------------------------------------
+
+enum ScanKind { SCAN_SEQUENTIAL, SCAN_DC_FIRST, SCAN_DC_REFINE, SCAN_AC_FIRST, SCAN_AC_REFINE };
+
+struct ScanDesc {                    // one scan of one multi-scan image
+  int img, kind, ncomp;
+  int comp[3], dc[3], ac[3];         // frame component indices in scan order; indices into the batch's Huffman tables
+  int ss, se, al;
+  int cols;                          // MCUs per row: the frame's when interleaved, else the component's blocks
+};
+
+struct MSeg {                        // one entropy-coded segment of a scan
+  long long start, end;
+  int scan, mcu0, nmcu;
+};
+
+__host__ __device__ __forceinline__ void refine_bit(BitReader& br, int16_t* c, int p1) {
+  if (br.nbits < 16) br.fill();
+  const int v = *c;
+  if (br.get(1) && !(v & p1)) *c = (int16_t)(v >= 0 ? v + p1 : v - p1);
+}
+
+// Decodes the blocks of one segment of a multi-scan file into the image's zero-initialised coefficients, with
+// libjpeg-turbo's jdhuff.c (sequential) and jdphuff.c (progressive) arithmetic.  Every coefficient is read and written
+// on its own: scans of the same dependency level update different coefficients of the same blocks concurrently.
+// Returns 0 or the segment's PG_JPEG_* error.
+__host__ __device__ inline int decode_scan_segment(const uint8_t* __restrict__ bytes, const ImgDesc& im,
+                                                   const HuffTbl* __restrict__ tbls, const ScanDesc& sc, const MSeg& sg,
+                                                   int16_t* __restrict__ coef) {
+#ifdef __CUDA_ARCH__
+  const uint8_t* natural = c_natural;
+#else
+  const uint8_t* natural = h_natural;
+#endif
+  BitReader br{bytes + sg.start, bytes + sg.end, 0, 0, 0, 0};
+  int pred0 = 0, pred1 = 0, pred2 = 0;
+  int eobrun = 0;
+  const int p1 = 1 << sc.al;
+  for (int mi = 0; mi < sg.nmcu && !br.err; ++mi) {
+    const int mcu = sg.mcu0 + mi;
+    const int my = mcu / sc.cols, mx = mcu - my * sc.cols;
+    for (int j = 0; j < sc.ncomp && !br.err; ++j) {
+      const Comp& cp = im.c[sc.comp[j]];
+      const int nv = sc.ncomp > 1 ? cp.v : 1, nh = sc.ncomp > 1 ? cp.h : 1;
+      for (int bv = 0; bv < nv && !br.err; ++bv)
+        for (int bh = 0; bh < nh && !br.err; ++bh) {
+          const long long b = cp.coef_off + (long long)(my * nv + bv) * cp.bw + (mx * nh + bh);
+          int16_t* blk = coef + b * 64;
+          if (sc.kind == SCAN_DC_REFINE) {
+            if (br.nbits < 16) br.fill();
+            if (br.get(1)) blk[0] = (int16_t)(blk[0] | p1);
+            continue;
+          }
+          if (sc.kind == SCAN_SEQUENTIAL || sc.kind == SCAN_DC_FIRST) {
+            if (br.nbits < 32) br.fill();
+            int s = huff_decode(br, tbls[sc.dc[j]]);
+            if (br.err) break;
+            if (s) s = huff_extend(br.get(s), s);
+            // predictor of scan component j, kept in registers (an indexed array would live in local memory)
+            const int pv = (j == 0 ? pred0 : j == 1 ? pred1 : pred2) + s;
+            if (j == 0) pred0 = pv; else if (j == 1) pred1 = pv; else pred2 = pv;
+            blk[0] = (int16_t)((unsigned)pv << sc.al);
+            if (sc.kind == SCAN_DC_FIRST) continue;
+          }
+          const HuffTbl& act = tbls[sc.ac[j]];
+          if (sc.kind != SCAN_AC_REFINE) {           // sequential AC, or the first scan of a band
+            if (eobrun > 0) { --eobrun; continue; }
+            for (int k = sc.kind == SCAN_SEQUENTIAL ? 1 : sc.ss; k <= sc.se; ++k) {
+              if (br.nbits < 32) br.fill();
+              const int rs = huff_decode(br, act);
+              if (br.err) break;
+              const int r = rs >> 4, s = rs & 15;
+              if (s) {
+                k += r;
+                if (k > sc.se) { br.err = ST_BAD_CODE; break; }
+                blk[natural[k]] = (int16_t)((unsigned)huff_extend(br.get(s), s) << sc.al);
+              } else if (r == 15) {
+                k += 15;
+              } else {
+                if (sc.kind == SCAN_SEQUENTIAL) break;
+                eobrun = (1 << r) - 1;
+                if (r) eobrun += br.get(r);
+                break;
+              }
+            }
+            continue;
+          }
+          int k = sc.ss;                              // decode_mcu_AC_refine
+          if (eobrun == 0) {
+            for (; k <= sc.se; ++k) {
+              if (br.nbits < 32) br.fill();
+              const int rs = huff_decode(br, act);
+              if (br.err) break;
+              int r = rs >> 4, s = rs & 15;
+              if (s) {
+                s = br.get(1) ? p1 : -p1;              // a newly nonzero coefficient is +-1 at this bit
+              } else if (r != 15) {
+                eobrun = 1 << r;
+                if (r) eobrun += br.get(r);
+                break;
+              }
+              // skip r zero coefficients, appending a correction bit to every nonzero one on the way
+              for (; k <= sc.se; ++k) {
+                int16_t* c = blk + natural[k];
+                if (*c) refine_bit(br, c, p1);
+                else if (--r < 0) break;
+              }
+              if (s) {
+                if (k > sc.se) { br.err = ST_BAD_CODE; break; }
+                blk[natural[k]] = (int16_t)s;
+              }
+            }
+          }
+          if (eobrun > 0 && !br.err) {                // the rest of the band: correction bits only
+            for (; k <= sc.se; ++k) {
+              int16_t* c = blk + natural[k];
+              if (*c) refine_bit(br, c, p1);
+            }
+            --eobrun;
+          }
+        }
+    }
+    if (!br.err && br.overrun()) br.err = ST_OVERRUN;
+  }
+  return br.err;
+}
+
+// One thread per segment of the launch's dependency level, packed into warps as in entropy_kernel.  A segment of an
+// image that an earlier level (or another segment) has already failed is skipped.
+__global__ void __launch_bounds__(ENTROPY_THREADS, 1)
+multiscan_kernel(const uint8_t* __restrict__ bytes, const ImgDesc* __restrict__ imgs, const HuffTbl* __restrict__ tbls,
+                 const ScanDesc* __restrict__ scans, const MSeg* __restrict__ segs, int nseg, int lanes,
+                 int16_t* __restrict__ coef, int* __restrict__ status) {
+  const int lane = threadIdx.x;
+  if (lane >= lanes) return;
+  const int si = blockIdx.x * lanes + lane;
+  if (si >= nseg) return;
+  const MSeg sg = segs[si];
+  const ScanDesc& sc = scans[sg.scan];
+  const ImgDesc& im = imgs[sc.img];
+  if (*(volatile const int*)(status + im.orig)) return;
+  const int err = decode_scan_segment(bytes, im, tbls, sc, sg, coef);
   if (err) atomicCAS(status + im.orig, 0, err);
 }
 
@@ -667,17 +1029,96 @@ struct Plan {
   std::vector<Seg> segs;
   std::vector<PlaneWork> planes;
   std::vector<long long> pix0;
+  std::vector<ScanDesc> scans;                        // multi-scan images
+  std::vector<MSeg> msegs;                            // their segments, ordered by dependency level
+  std::vector<int> level0;                            // msegs of level L: [level0[L - 1], level0[L])
   long long nblocks = 0, plane_bytes = 0, npix = 0;
-  size_t off_imgs = 0, off_tbls = 0, off_segs = 0, off_planes = 0, off_pix0 = 0, meta_bytes = 0;
+  long long multi_coef0 = -1, multi_coef1 = -1;       // blocks [multi_coef0, multi_coef1) hold every multi-scan image
+  size_t off_imgs = 0, off_tbls = 0, off_segs = 0, off_planes = 0, off_pix0 = 0, off_scans = 0, off_msegs = 0,
+         meta_bytes = 0;
   size_t off_bytes = 0, off_meta = 0, off_coef = 0, off_plane = 0, total = 0;
 };
+
+// Index of the Huffman table (bits, vals) in the batch's de-duplicated table array; -1 for an invalid table.
+int huff_index(std::map<std::string, int>& index, std::vector<HuffTbl>& tbls, const uint8_t* bits, const uint8_t* vals,
+               int cls) {
+  std::string key(1, (char)cls);
+  key.append((const char*)bits, 16);
+  key.append((const char*)vals, 256);
+  auto it = index.find(key);
+  if (it != index.end()) return it->second;
+  const int idx = (int)tbls.size();
+  tbls.emplace_back();
+  if (!make_huff(bits, vals, cls == 0, &tbls.back())) return -1;
+  index.emplace(key, idx);
+  return idx;
+}
+
+// The scans of multi-scan image k (file bytes [base, base + len) of the packed input), found again by the multi-scan
+// walk that validated them: their descriptors, segments (by level), latched quantisation tables and Huffman tables.
+int plan_multiscan(const uint8_t* packed, int64_t base, int64_t len, const pg_jpeg_info& in, int i, int k, ImgDesc& d,
+                   std::map<std::string, int>& tbl_index, std::vector<std::vector<MSeg>>& by_level, Plan* P) {
+  MultiScan ms;
+  ms.want_segs = true;
+  pg_jpeg_info w;
+  char msg[200];
+  Why why{msg, sizeof(msg)};
+  if (parse_multiscan(packed + base, len, &w, &ms, &why) != PG_JPEG_OK || !(w.table_mask & PG_JPEG_MULTISCAN) ||
+      w.width != in.width || w.height != in.height || w.components != in.components ||
+      w.num_segments != in.num_segments || memcmp(w.h_samp, in.h_samp, sizeof(w.h_samp)) ||
+      memcmp(w.v_samp, in.v_samp, sizeof(w.v_samp))) {
+    set_last_error("jpeg: image %d does not match its pg_jpeg_info", i);
+    return 1;
+  }
+  for (int c = 0; c < d.ncomp; ++c)
+    for (int q = 0; q < 64; ++q) d.c[c].q[h_natural[q]] = (int16_t)ms.qt[c][q];
+  const bool progressive = w.sof == 0xC2;
+  for (const ScanRec& r : ms.scans) {
+    const pg_jpeg_scan& p = r.pub;
+    ScanDesc sd;
+    memset(&sd, 0, sizeof(sd));
+    sd.img = k;
+    sd.kind = !progressive ? SCAN_SEQUENTIAL
+              : p.ss == 0  ? (p.ah ? SCAN_DC_REFINE : SCAN_DC_FIRST)
+                           : (p.ah ? SCAN_AC_REFINE : SCAN_AC_FIRST);
+    sd.ncomp = p.components;
+    sd.ss = p.ss; sd.se = p.se; sd.al = p.al;
+    int rows = 0;
+    scan_grid(&w, p.components, p.component[0], &sd.cols, &rows);
+    for (int j = 0; j < p.components; ++j) {
+      sd.comp[j] = p.component[j];
+      const bool need_dc = sd.kind == SCAN_SEQUENTIAL || sd.kind == SCAN_DC_FIRST;
+      const bool need_ac = sd.kind == SCAN_SEQUENTIAL || sd.kind == SCAN_AC_FIRST || sd.kind == SCAN_AC_REFINE;
+      sd.dc[j] = need_dc ? huff_index(tbl_index, P->tbls, r.dc_bits[j], r.dc_vals[j], 0) : 0;
+      sd.ac[j] = need_ac ? huff_index(tbl_index, P->tbls, r.ac_bits[j], r.ac_vals[j], 1) : 0;
+      if (sd.dc[j] < 0 || sd.ac[j] < 0) {
+        set_last_error("jpeg: image %d has an invalid Huffman table", i);
+        return 1;
+      }
+    }
+    const int total = sd.cols * rows;
+    const int ri = p.restart_interval ? p.restart_interval : total;
+    if ((int)by_level.size() < p.level) by_level.resize(p.level);
+    for (int s = 0; s < p.num_segments; ++s) {
+      MSeg sg;
+      sg.start = base + r.segs[s].first;
+      sg.end = base + r.segs[s].second;
+      sg.scan = (int)P->scans.size();
+      sg.mcu0 = s * ri;
+      sg.nmcu = std::min(ri, total - sg.mcu0);
+      by_level[p.level - 1].push_back(sg);
+    }
+    P->scans.push_back(sd);
+  }
+  return 0;
+}
 
 // Sizes every region from the parse results; with `packed` it also fills the tables the kernels read.
 int make_plan(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info* infos, int n, int64_t packed_bytes,
               const pg_image* dst, Plan* P) {
   if (n <= 0 || !infos || packed_bytes < 0) { set_last_error("jpeg: bad argument"); return 1; }
   std::map<std::string, int> tbl_index;
-  long long segs = 0;
+  long long segs = 0, msegs = 0, mtables = 0;
   for (int i = 0; i < n; ++i) {
     const pg_jpeg_info& in = infos[i];
     if (in.status != PG_JPEG_OK) continue;
@@ -685,6 +1126,7 @@ int make_plan(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info*
       set_last_error("jpeg: image %d has an inconsistent pg_jpeg_info", i);
       return 1;
     }
+    const bool multi = (in.table_mask & PG_JPEG_MULTISCAN) != 0;
     ImgDesc d;
     memset(&d, 0, sizeof(d));
     d.orig = i;
@@ -703,29 +1145,22 @@ int make_plan(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info*
       cp.dh = (int)(((long long)in.height * cp.v + d.vmax - 1) / d.vmax);
       cp.coef_off = P->nblocks;
       cp.plane_off = P->plane_bytes;
+      if (multi && c == 0 && P->multi_coef0 < 0) P->multi_coef0 = P->nblocks;
       P->planes.push_back({P->nblocks, (int)P->imgs.size(), c});
       P->nblocks += (long long)cp.bw * cp.bh;
       P->plane_bytes += (long long)align_up((size_t)cp.bw * cp.bh * 64, 16);
+      if (multi) {                                    // tables per scan: plan_multiscan
+        P->multi_coef1 = P->nblocks;
+        continue;
+      }
       for (int k = 0; k < 64; ++k) cp.q[h_natural[k]] = (int16_t)in.qt[in.quant_table[c]][k];
       for (int cls = 0; cls < 2; ++cls) {
         const int th = cls ? in.ac_table[c] : in.dc_table[c];
-        const uint8_t* bits = cls ? in.ac_bits[th] : in.dc_bits[th];
-        const uint8_t* vals = cls ? in.ac_vals[th] : in.dc_vals[th];
-        std::string key(1, (char)cls);
-        key.append((const char*)bits, 16);
-        key.append((const char*)vals, 256);
-        auto it = tbl_index.find(key);
-        int idx;
-        if (it == tbl_index.end()) {
-          idx = (int)P->tbls.size();
-          P->tbls.emplace_back();
-          if (!make_huff(bits, vals, cls == 0, &P->tbls.back())) {
-            set_last_error("jpeg: image %d has an invalid Huffman table", i);
-            return 1;
-          }
-          tbl_index.emplace(key, idx);
-        } else {
-          idx = it->second;
+        const int idx = huff_index(tbl_index, P->tbls, cls ? in.ac_bits[th] : in.dc_bits[th],
+                                   cls ? in.ac_vals[th] : in.dc_vals[th], cls);
+        if (idx < 0) {
+          set_last_error("jpeg: image %d has an invalid Huffman table", i);
+          return 1;
         }
         (cls ? cp.ac : cp.dc) = idx;
       }
@@ -740,16 +1175,53 @@ int make_plan(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info*
     }
     P->pix0.push_back(P->npix);
     P->npix += (long long)in.width * in.height;
-    segs += in.num_segments;
+    if (multi) {
+      msegs += in.num_segments;
+      mtables += (unsigned)in.table_mask >> 16;
+    } else {
+      segs += in.num_segments;
+    }
     P->imgs.push_back(d);
   }
+  // Without the files, the multi-scan regions are sized by bounds from the infos: a scan has at least one segment,
+  // and the batch has no more Huffman tables than selections.
+  std::vector<std::vector<MSeg>> by_level;
+  if (packed) {
+    int k = 0;
+    for (int i = 0; i < n; ++i) {
+      const pg_jpeg_info& in = infos[i];
+      if (in.status != PG_JPEG_OK) continue;
+      if (in.table_mask & PG_JPEG_MULTISCAN) {
+        const int64_t base = offsets[i], len = offsets[i + 1] - offsets[i];
+        if (base < 0 || len < 0 || offsets[i + 1] > packed_bytes) {
+          set_last_error("jpeg: image %d lies outside the packed input", i);
+          return 1;
+        }
+        if (plan_multiscan(packed, base, len, in, i, k, P->imgs[k], tbl_index, by_level, P)) return 1;
+      }
+      ++k;
+    }
+    P->level0.push_back(0);
+    for (auto& v : by_level) {
+      P->msegs.insert(P->msegs.end(), v.begin(), v.end());
+      P->level0.push_back((int)P->msegs.size());
+    }
+    if ((long long)P->msegs.size() != msegs) {
+      set_last_error("jpeg: the multi-scan images do not match their pg_jpeg_info");
+      return 1;
+    }
+  }
   const size_t nimg = P->imgs.size();
+  const size_t ntbls = packed ? P->tbls.size() : P->tbls.size() + (size_t)mtables;
+  const size_t nscans = packed ? P->scans.size() : (size_t)msegs;
   size_t off = 0;
   P->off_imgs = off; off += align_up(nimg * sizeof(ImgDesc), 256);
-  P->off_tbls = off; off += align_up(P->tbls.size() * sizeof(HuffTbl), 256);
+  P->off_tbls = off; off += align_up(ntbls * sizeof(HuffTbl), 256);
   P->off_segs = off; off += align_up((size_t)segs * sizeof(Seg), 256);
   P->off_planes = off; off += align_up(P->planes.size() * sizeof(PlaneWork), 256);
   P->off_pix0 = off; off += align_up(nimg * sizeof(long long), 256);
+  P->off_scans = off; off += align_up(nscans * sizeof(ScanDesc), 256);
+  P->off_msegs = off; off += align_up((size_t)msegs * sizeof(MSeg), 256);
   P->meta_bytes = off;
   size_t total = 0;
   P->off_bytes = total; total += align_up((size_t)packed_bytes, 256);
@@ -763,6 +1235,7 @@ int make_plan(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info*
   for (int i = 0; i < n; ++i) {
     const pg_jpeg_info& in = infos[i];
     if (in.status != PG_JPEG_OK) continue;
+    if (in.table_mask & PG_JPEG_MULTISCAN) { ++k; continue; }
     const ImgDesc& d = P->imgs[k];
     const int64_t base = offsets[i], len = offsets[i + 1] - offsets[i];
     if (base < 0 || len < 0 || offsets[i + 1] > packed_bytes || in.scan_offset < 0 || in.scan_bytes < 0 ||
@@ -807,6 +1280,45 @@ int jpeg_parse(const uint8_t* data, int64_t bytes, pg_jpeg_info* info) {
   return st;
 }
 
+int jpeg_parse_multiscan(const uint8_t* data, int64_t bytes, pg_jpeg_info* info) {
+  if (!info) { set_last_error("pg_jpeg_parse_multiscan: null info"); return -1; }
+  char msg[200];
+  Why why{msg, sizeof(msg)};
+  msg[0] = 0;
+  MultiScan ms;
+  const int st = parse_multiscan(data, bytes, info, &ms, &why);
+  if (st) set_last_error("%s", msg);
+  return st;
+}
+
+int jpeg_scans(const uint8_t* data, int64_t bytes, pg_jpeg_scan* out, int cap) {
+  char msg[200];
+  Why why{msg, sizeof(msg)};
+  msg[0] = 0;
+  MultiScan ms;
+  pg_jpeg_info info;
+  if (parse_multiscan(data, bytes, &info, &ms, &why) != PG_JPEG_OK) {
+    set_last_error("%s", msg);
+    return -1;
+  }
+  std::vector<pg_jpeg_scan> scans;
+  if (info.table_mask & PG_JPEG_MULTISCAN) {
+    for (const ScanRec& r : ms.scans) scans.push_back(r.pub);
+  } else {                                            // a single-scan file, as pg_jpeg_parse describes it
+    pg_jpeg_scan p;
+    memset(&p, 0, sizeof(p));
+    p.components = info.components;
+    for (int c = 0; c < info.components; ++c) p.component[c] = c;
+    p.se = 63;
+    p.restart_interval = info.restart_interval;
+    p.num_segments = info.num_segments;
+    p.level = 1;
+    scans.push_back(p);
+  }
+  for (int i = 0; i < (int)scans.size() && i < cap && out; ++i) out[i] = scans[i];
+  return (int)scans.size();
+}
+
 size_t jpeg_workspace_bytes(const pg_jpeg_info* infos, int n, int64_t packed_bytes) {
   Plan P;
   if (make_plan(nullptr, nullptr, infos, n, packed_bytes, nullptr, &P)) return 0;
@@ -833,6 +1345,8 @@ int jpeg_decode(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_inf
   memcpy(meta.data() + P.off_segs, P.segs.data(), P.segs.size() * sizeof(Seg));
   memcpy(meta.data() + P.off_planes, P.planes.data(), P.planes.size() * sizeof(PlaneWork));
   memcpy(meta.data() + P.off_pix0, P.pix0.data(), nimg * sizeof(long long));
+  memcpy(meta.data() + P.off_scans, P.scans.data(), P.scans.size() * sizeof(ScanDesc));
+  memcpy(meta.data() + P.off_msegs, P.msegs.data(), P.msegs.size() * sizeof(MSeg));
   std::vector<int32_t> host_status(n);   // the parse status of skipped images, 0 for the ones the kernels decode
   for (int i = 0; i < n; ++i) host_status[i] = infos[i].status;
   cudaError_t e = cudaMemcpyAsync(ws + P.off_bytes, packed, (size_t)offsets[n], cudaMemcpyHostToDevice, stream);
@@ -857,11 +1371,36 @@ int jpeg_decode(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_inf
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   }
   // one segment per warp until every SM holds 16 warps, then pack lanes
-  const int lanes = (int)std::min<long long>(ENTROPY_THREADS, std::max<long long>(1, (nseg + 16LL * sms - 1) / (16LL * sms)));
-  {
+  auto lanes_for = [sms](long long segs) {
+    return (int)std::min<long long>(ENTROPY_THREADS, std::max<long long>(1, (segs + 16LL * sms - 1) / (16LL * sms)));
+  };
+  if (!P.msegs.empty()) {
+    // before any entropy launch: the range of multi-scan blocks may hold baseline images between them
+    ProfScope prof("jpeg_zero_coef", stream);
+    e = cudaMemsetAsync(d_coef + P.multi_coef0 * 64, 0, (size_t)(P.multi_coef1 - P.multi_coef0) * 128, stream);
+    if (e != cudaSuccess) { set_last_error("pg_jpeg_decode: memset: %s", cudaGetErrorString(e)); return 1; }
+  }
+  if (nseg > 0) {
+    const int lanes = lanes_for(nseg);
     ProfScope prof("jpeg_entropy", stream);
     entropy_kernel<<<(nseg + lanes - 1) / lanes, ENTROPY_THREADS, 0, stream>>>(ws + P.off_bytes, d_imgs, d_tbls, d_segs,
                                                                                 nseg, lanes, d_coef, status_out);
+  }
+  if (!P.msegs.empty()) {
+    // Multi-scan images (coefficients zeroed above): one launch per dependency level.  The scans of one level share
+    // no coefficient; a later level reads what earlier ones wrote, ordered by the stream alone.
+    static const char* level_names[] = {"jpeg_entropy_multiscan.1", "jpeg_entropy_multiscan.2", "jpeg_entropy_multiscan.3",
+                                        "jpeg_entropy_multiscan.4", "jpeg_entropy_multiscan.5+"};
+    const ScanDesc* d_scans = reinterpret_cast<const ScanDesc*>(meta_d + P.off_scans);
+    const MSeg* d_msegs = reinterpret_cast<const MSeg*>(meta_d + P.off_msegs);
+    for (size_t L = 0; L + 1 < P.level0.size(); ++L) {
+      const int s0 = P.level0[L], ns = P.level0[L + 1] - s0;
+      if (ns == 0) continue;
+      const int lanes = lanes_for(ns);
+      ProfScope prof(level_names[std::min<size_t>(L, 4)], stream);
+      multiscan_kernel<<<(ns + lanes - 1) / lanes, ENTROPY_THREADS, 0, stream>>>(
+          ws + P.off_bytes, d_imgs, d_tbls, d_scans, d_msegs + s0, ns, lanes, d_coef, status_out);
+    }
   }
   {
     ProfScope prof("jpeg_idct", stream);
@@ -881,6 +1420,14 @@ int jpeg_decode(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_inf
 
 extern "C" int pg_jpeg_parse(const uint8_t* data_host, int64_t bytes, pg_jpeg_info* info_out) {
   return pg::jpeg_parse(data_host, bytes, info_out);
+}
+
+extern "C" int pg_jpeg_parse_multiscan(const uint8_t* data_host, int64_t bytes, pg_jpeg_info* info_out) {
+  return pg::jpeg_parse_multiscan(data_host, bytes, info_out);
+}
+
+extern "C" int pg_jpeg_scans(const uint8_t* data_host, int64_t bytes, pg_jpeg_scan* out, int32_t cap) {
+  return pg::jpeg_scans(data_host, bytes, out, cap);
 }
 
 extern "C" size_t pg_jpeg_workspace_bytes(const pg_jpeg_info* infos_host, int32_t n, int64_t packed_bytes) {

@@ -8,6 +8,10 @@ pretrain_dataset.py:109-161).
 The headers are parsed on the host (`parse`); the compressed bytes of the whole batch go to the device in one copy and
 three launches decode them.  Files outside the decoded subset (progressive, 12-bit, CMYK, RGB-transform, other
 sampling layouts) and corrupt files raise `ValueError` naming every such index and its reason.
+
+With `multiscan=True`, progressive files and sequential files of several scans are decoded too, to the same bytes as
+Pillow, when every coefficient is sent and fully refined (what encoders write; libjpeg smooths the blocks of the other
+ones, which are refused).  Their scans decode in one launch per dependency level (`scans(data)` lists them).
 """
 from __future__ import annotations
 
@@ -21,6 +25,8 @@ from . import _lib
 from ._lib import PigeonB200Error, check, current_stream_ptr, load
 
 OK, UNSUPPORTED, BAD_HEADER, BAD_CODE, OVERRUN, UNEXPECTED_MARKER, BAD_RST, NO_EOI = range(8)
+MULTISCAN = 1 << 12          # PG_JPEG_MULTISCAN
+MAX_SCANS = 256              # PG_JPEG_MAX_SCANS
 STATUS_TEXT = {OK: "ok", UNSUPPORTED: "not decoded by this decoder", BAD_HEADER: "truncated or inconsistent header",
                BAD_CODE: "corrupt entropy data: code missing from its Huffman table",
                OVERRUN: "corrupt entropy data: a segment ends before its MCUs",
@@ -40,13 +46,33 @@ class JpegDecodeError(ValueError):
         self.images = images
 
 
-def parse(data: Encoded) -> Tuple[_lib.JpegInfo, str]:
-    """Host marker walk of one file: its `pg_jpeg_info` and, when its status is not OK, the reason."""
+def parse(data: Encoded, multiscan: bool = False) -> Tuple[_lib.JpegInfo, str]:
+    """Host marker walk of one file: its `pg_jpeg_info` and, when its status is not OK, the reason.  `multiscan` also
+    accepts progressive and multi-scan sequential files (pg_jpeg_parse_multiscan); a single-scan file gets the same
+    info either way."""
     lib = load()
     buf = bytes(data)
     info = _lib.JpegInfo()
-    st = lib.pg_jpeg_parse(buf, len(buf), C.byref(info))
+    fn = lib.pg_jpeg_parse_multiscan if multiscan else lib.pg_jpeg_parse
+    st = fn(buf, len(buf), C.byref(info))
     return info, ("" if st == OK else lib.pg_last_error().decode())
+
+
+def is_multiscan(info: _lib.JpegInfo) -> bool:
+    """True for the info of a progressive or multi-scan file (the PG_JPEG_MULTISCAN bit of table_mask)."""
+    return bool(info.table_mask & MULTISCAN)
+
+
+def scans(data: Encoded) -> List[_lib.JpegScan]:
+    """The scans of a file that `parse(data, multiscan=True)` accepts, in file order: components, Ss, Se, Ah, Al,
+    restart interval, segment count and dependency level.  ValueError with the reason for a refused file."""
+    lib = load()
+    buf = bytes(data)
+    out = (_lib.JpegScan * MAX_SCANS)()
+    n = lib.pg_jpeg_scans(buf, len(buf), out, MAX_SCANS)
+    if n < 0:
+        raise ValueError(lib.pg_last_error().decode())
+    return list(out[:n])
 
 
 class JpegDecoder:
@@ -60,16 +86,18 @@ class JpegDecoder:
         self._ws = None
         self._pinned = None        # staging of the compressed bytes; free again once the status has been read back
 
-    def decode(self, files: Sequence[Encoded], infos: Sequence[_lib.JpegInfo] = None) -> List[torch.Tensor]:
+    def decode(self, files: Sequence[Encoded], infos: Sequence[_lib.JpegInfo] = None,
+               multiscan: bool = False) -> List[torch.Tensor]:
         """files -> CUDA uint8 [H, W, 3] views into one arena (Pillow's `.convert('RGB')` bytes).  `infos` are the
-        `parse` results when the caller already has them.  Raises JpegDecodeError (a ValueError) listing every rejected
-        or corrupt index; the other files of the batch are still decoded."""
+        `parse` results when the caller already has them (multi-scan infos are decoded whatever `multiscan` says);
+        otherwise the files are parsed with `parse(f, multiscan)`.  Raises JpegDecodeError (a ValueError) listing every
+        rejected or corrupt index; the other files of the batch are still decoded."""
         n = len(files)
         if n == 0:
             return []
         bufs = [memoryview(f).cast("B") for f in files]
         if infos is None:
-            parsed = [parse(b) for b in bufs]
+            parsed = [parse(b, multiscan) for b in bufs]
             infos = [p[0] for p in parsed]
             reasons = [p[1] for p in parsed]
         else:
@@ -111,6 +139,7 @@ class JpegDecoder:
         return images
 
 
-def decode_jpeg(files: Sequence[Encoded], device: Union[str, torch.device] = "cuda") -> List[torch.Tensor]:
-    """One-shot `JpegDecoder(device).decode(files)`."""
-    return JpegDecoder(device).decode(files)
+def decode_jpeg(files: Sequence[Encoded], device: Union[str, torch.device] = "cuda",
+                multiscan: bool = False) -> List[torch.Tensor]:
+    """One-shot `JpegDecoder(device).decode(files, multiscan=multiscan)`."""
+    return JpegDecoder(device).decode(files, multiscan=multiscan)

@@ -10,6 +10,8 @@ Images may also be encoded files (`bytes` / `bytearray` / `memoryview`).  Baseli
 (pigeon_b200.jpeg, one decode launch sequence per call); every other encoded file (PNG, progressive JPEG, anything the
 JPEG parser does not decode) is decoded by Pillow on the host, the reference's own decoder, so the pixels are the same
 either way.  `gpu_decoded` / `host_decoded` count the two routes.  A JPEG with corrupt entropy-coded data raises.
+`jpeg_multiscan=True` sends progressive and multi-scan JPEGs to the GPU decoder as well (opt-in until it is measured at
+least as fast as the host route on progressive photos; DESIGN.md §1).
 """
 from __future__ import annotations
 
@@ -39,10 +41,11 @@ def _to_u8_rgb(img) -> np.ndarray:
     return np.ascontiguousarray(img)
 
 
-def route_encoded(data) -> tuple:
+def route_encoded(data, multiscan: bool = False) -> tuple:
     """('gpu', info) for a file the GPU JPEG decoder takes, ('host', info) for one Pillow decodes on the host (PNG,
-    progressive JPEG, anything else the parser does not decode); ValueError for a JPEG with corrupt entropy data."""
-    info, reason = jpeg.parse(data)
+    progressive JPEG unless `multiscan`, anything else the parser does not decode); ValueError for a JPEG with corrupt
+    entropy data."""
+    info, reason = jpeg.parse(data, multiscan)
     if info.status == jpeg.OK:
         return "gpu", info
     if info.status in (jpeg.UNSUPPORTED, jpeg.BAD_HEADER):
@@ -52,11 +55,14 @@ def route_encoded(data) -> tuple:
 
 class ClipImageProcessor:
     """Call-compatible with the way the reference uses `CLIPProcessor` for images: `proc(images=..., return_tensors='pt')`
-    returns a dict with 'pixel_values' (here a CUDA tensor).  `dtype=torch.float16` writes the tower's input type directly."""
+    returns a dict with 'pixel_values' (here a CUDA tensor).  `dtype=torch.float16` writes the tower's input type directly.
+    `jpeg_multiscan=True` decodes encoded progressive and multi-scan JPEGs on the GPU instead of with Pillow."""
 
     def __init__(self, size: int = 336, image_mean: Sequence[float] = CLIP_MEAN, image_std: Sequence[float] = CLIP_STD,
-                 device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float32):
+                 device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float32,
+                 jpeg_multiscan: bool = False):
         self.size = int(size)
+        self.jpeg_multiscan = bool(jpeg_multiscan)
         self.mean = np.asarray(image_mean, dtype=np.float64).astype(np.float32)
         self.std = np.asarray(image_std, dtype=np.float64).astype(np.float32)
         self.device = torch.device(device)
@@ -103,7 +109,7 @@ class ClipImageProcessor:
                 continue
             if isinstance(img, (bytes, bytearray, memoryview)):
                 try:
-                    route, info = route_encoded(img)
+                    route, info = route_encoded(img, self.jpeg_multiscan)
                 except ValueError as e:
                     raise ValueError(f"image {i}: {e}") from None
                 if route == "gpu":

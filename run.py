@@ -2,7 +2,7 @@
 """Entry points of the hot path with the reference's CLI (run.py:21-93): `embed`, `evaluate` and `finetune`.
 
     python run.py evaluate HEAD.model -l DATASET_DIR [-b BASE.model] [--yfcc] [--metrics]
-    python run.py embed CLIP.model -l DATASET_DIR                                                # image column + index
+    python run.py embed CLIP.model -l DATASET_DIR [--jpeg-multiscan]                             # image column + index
     python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading]     # tower + head (run.py:165-169)
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
 
@@ -83,6 +83,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument('--heading', action='store_true')
     p.add_argument('-m', '--multitask', action='store_true')
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
+    p.add_argument('--jpeg-multiscan', action='store_true',
+                   help='embed: decode progressive and multi-scan JPEGs on the GPU too (by default Pillow decodes them)')
     p.add_argument('--metrics', action='store_true',
                    help='evaluate / finetune: report compute_geoguessr_metrics (needs config.COUNTRY_PATH)')
     return p
@@ -116,7 +118,11 @@ def main(argv=None):
             finetune_model(args.name, ds, multi_task=args.multitask, heading=args.heading, yfcc=args.yfcc,
                            metrics=metrics_fn(args))                                                          # run.py:169
     elif args.mode == 'embed':
-        model = CLIPEmbedding(args.name, load_checkpoint=True, panorama=not args.yfcc)    # run.py:126-129
+        kw = {}
+        if args.jpeg_multiscan:
+            from pigeon_b200.preprocess import ClipImageProcessor
+            kw['processor'] = ClipImageProcessor(device='cuda', dtype=torch.float16, jpeg_multiscan=True)
+        model = CLIPEmbedding(args.name, load_checkpoint=True, panorama=not args.yfcc, **kw)    # run.py:126-129
         # EmbedDataset semantics (embed_dataset.py:17-22): data['image'] and data['index'] of each split; the files stay
         # encoded until the GPU decodes them
         from datasets import Image

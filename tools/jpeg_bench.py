@@ -8,7 +8,11 @@ kernel times (CUDA events around each launch), and the host-to-device bytes.  Fo
 host core followed by the same GPU pre-processing, and a CLIPEmbedding (ViT-L/14-336) pass from bytes against the same
 pass from pre-decoded host pixels.  Prints one JSON line per measurement.
 
-    python tools/jpeg_bench.py [--iters 10] [--warmup 3] [--out DIR]
+`--multiscan` measures instead the progressive versions of the two corpora (Pillow's progressive=True, libjpeg's
+10-scan script, no restart markers) through the multi-scan path (`jpeg_multiscan=True`), with the kernel time of each
+dependency level, against the host route (Pillow on every host core + the same GPU pre-processing).
+
+    python tools/jpeg_bench.py [--multiscan] [--iters 10] [--warmup 3] [--out DIR]
 """
 import argparse
 import ctypes as C
@@ -38,13 +42,16 @@ def card():
     return name, power
 
 
-def corpus(h, w, q, restart, distinct=16):
-    from PIL import Image
+def corpus(h, w, q, restart, distinct=16, progressive=False):
+    from PIL import Image, ImageFile
     from pigeon_b200 import synthetic
+    ImageFile.MAXBLOCK = max(ImageFile.MAXBLOCK, 1 << 24)      # Pillow's progressive encoder buffers the whole file
     out = []
     for i in range(distinct):
         f = io.BytesIO()
         kw = dict(restart_marker_rows=1) if restart else {}
+        if progressive:
+            kw["progressive"] = True
         Image.fromarray(synthetic.synthetic_photo(h, w, seed=1000 + i)).save(f, "JPEG", quality=q, subsampling=2, **kw)
         out.append(f.getvalue())
     return out
@@ -79,6 +86,7 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--out", default=None, help="also write the JSON lines to DIR/jpeg_bench.jsonl")
+    ap.add_argument("--multiscan", action="store_true", help="progressive corpora through the multi-scan path")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("jpeg_bench needs a CUDA device")
@@ -99,7 +107,9 @@ def main():
     dec = JpegDecoder(dev)
     proc = ClipImageProcessor(device=dev, dtype=torch.float16)
     corpora = {"640x640 q90": (640, 640, 90), "1024x768 q85": (768, 1024, 85)}
-    for cname, (h, w, q) in corpora.items():
+    if args.multiscan:
+        multiscan(args, dec, corpora, emit)
+    for cname, (h, w, q) in (corpora.items() if not args.multiscan else ()):
         for restart in (False, True):
             distinct = corpus(h, w, q, restart)
             for n in (64, 256, 1024):
@@ -126,7 +136,47 @@ def main():
             emit(dict(corpus=cname, restart_rows=restart, images=256, pillow_threads=cores,
                       pillow_decode_pre_ms=round(t * 1e3, 3), pillow_decode_pre_img_s=round(256 / t, 1)))
 
+    if not args.multiscan:
+        embedding(args, emit)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        name = "jpeg_bench_multiscan.jsonl" if args.multiscan else "jpeg_bench.jsonl"
+        with open(os.path.join(args.out, name), "w") as f:
+            f.write("".join(json.dumps(d) + "\n" for d in lines))
+
+
+def multiscan(args, dec, corpora, emit):
+    from PIL import Image
+    from pigeon_b200.preprocess import ClipImageProcessor
+    proc = ClipImageProcessor(device=dec.device, dtype=torch.float16, jpeg_multiscan=True)
+    cores = os.cpu_count()
+    for cname, (h, w, q) in corpora.items():
+        distinct = corpus(h, w, q, False, progressive=True)
+        for n in (64, 256, 1024):
+            files = [distinct[i % len(distinct)] for i in range(n)]
+            mb = sum(len(f) for f in files) / 1e6
+            t_dec = timed(lambda: dec.decode(files, multiscan=True), args.iters, args.warmup)
+            t_pre = timed(lambda: proc(images=files), args.iters, args.warmup)
+            stages = stage_ms(lambda: dec.decode(files, multiscan=True))
+            emit(dict(corpus=cname + " progressive", images=n, compressed_mb=round(mb, 3),
+                      decode_ms=round(t_dec * 1e3, 3), decode_img_s=round(n / t_dec, 1),
+                      decode_pre_ms=round(t_pre * 1e3, 3), decode_pre_img_s=round(n / t_pre, 1), stage_ms=stages))
+            pool = ThreadPoolExecutor(cores)
+            host = ClipImageProcessor(device=dec.device, dtype=torch.float16)
+
+            def pillow_then_gpu():
+                px = list(pool.map(lambda b: np.asarray(Image.open(io.BytesIO(b)).convert("RGB")), files))
+                return host(images=px)
+
+            t = timed(pillow_then_gpu, max(2, args.iters // 3), 1)
+            pool.shutdown()
+            emit(dict(corpus=cname + " progressive", images=n, pillow_threads=cores,
+                      pillow_decode_pre_ms=round(t * 1e3, 3), pillow_decode_pre_img_s=round(n / t, 1)))
+
+
+def embedding(args, emit):
     # CLIPEmbedding (ViT-L/14-336, random weights) from bytes against from pre-decoded host pixels, batch 64
+    from PIL import Image
     from pigeon_b200 import CLIPEmbedding, synthetic
     from pigeon_b200.super_guessr import CLIPVisionTower
     from pigeon_b200.vit_engine import VitDims
@@ -144,10 +194,6 @@ def main():
     t_px = timed(lambda: model(pixels), args.iters, args.warmup)
     emit(dict(workload="CLIPEmbedding ViT-L/14-336 batch 64, 640x640 q90", embeddings_identical=same,
               from_bytes_ms=round(t_bytes * 1e3, 3), from_host_pixels_ms=round(t_px * 1e3, 3)))
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "jpeg_bench.jsonl"), "w") as f:
-            f.write("".join(json.dumps(d) + "\n" for d in lines))
 
 
 if __name__ == "__main__":
