@@ -45,6 +45,9 @@ PROTO_PATH_LANDMARKS = 'data/data_prototypes_landmarks.csv'
 DATASET_PATH_LANDMARKS = 'data/hf_landmarks'
 PROTO_MODEL_LANDMARKS_PATH = 'saved_models/refiner/proto_landmarks.refiner'
 
+# Benchmarks: a JSON file supplied by the user, {name: {"meta": CSV path, "images": image folder prefix}}   (config.py:91)
+BENCHMARKS = 'data/benchmarks/benchmarks.json'
+
 # Evaluation batch size (TRAIN_ARGS.per_device_eval_batch_size)        (config.py:98)
 EVAL_BATCH_SIZE = 256
 

@@ -23,11 +23,17 @@ logger = logging.getLogger('evaluation')
 
 
 def evaluate_model(model, dataset, metrics: Optional[Callable], train_args=None, refiner=None, yfcc: bool = False,
-                   writer=None, step: int = 0, num_workers: int = 0):
-    """reference training/train_eval_loop.py:35-161.  `train_args` only needs `.per_device_eval_batch_size`."""
+                   writer=None, step: int = 0, num_workers: int = 0, collate_fn=None, processor=None):
+    """reference training/train_eval_loop.py:35-161.  `train_args` only needs `.per_device_eval_batch_size`.
+    With `collate_fn=encoded_eval_collate` and a `processor` (preprocess.ClipImageProcessor), `dataset` yields encoded
+    files (`BenchmarkDataset.encoded()`, `EvalDataset.encoded()`) and each batch is decoded and pre-processed on the
+    GPU before the model sees it; without them the batches carry pixel_values, as before."""
     logger.warning('Starting evaluation ...')
     bs = getattr(train_args, 'per_device_eval_batch_size', EVAL_BATCH_SIZE)
-    eval_data = DataLoader(dataset, bs, shuffle=False, pin_memory=True, num_workers=num_workers)
+    if (collate_fn is None) != (processor is None):
+        raise ValueError('collate_fn and processor go together: the collate yields encoded files, the processor decodes them')
+    eval_data = DataLoader(dataset, bs, shuffle=False, pin_memory=collate_fn is None, num_workers=num_workers,
+                           collate_fn=collate_fn)
     was_training = model.training
     model.eval()
     if refiner is not None:
@@ -35,6 +41,8 @@ def evaluate_model(model, dataset, metrics: Optional[Callable], train_args=None,
     preds, cells, top_cells, top_probs, losses, n = [], [], [], [], [], 0
     with torch.no_grad():
         for data in eval_data:                                                       # :77
+            if processor is not None:
+                data = encoded_pixel_values(data, processor)
             ll, cell, outputs = predict_batch(model, refiner, dict(data), gather=False)
             b = ll.shape[0]
             n += b
@@ -92,19 +100,40 @@ def raw_image_collate(batch):
     return list(images), torch.as_tensor(index)
 
 
+def read_encoded(image) -> bytes:
+    """The file behind an HF `Image(decode=False)` value ({'bytes', 'path'}): its bytes, or the file at its path when
+    the bytes are None."""
+    data = image.get('bytes')
+    if data is None:
+        with open(image['path'], 'rb') as f:
+            data = f.read()
+    return data
+
+
 def encoded_image_collate(batch):
     """collate_fn for rows of an HF dataset whose `image` column is cast to `Image(decode=False)` (the reference's
     EmbedDataset rows: data['image'], data['index']): yields (list of encoded files, index).  A row's `bytes` are used,
     or its `path` is read when `bytes` is None; the model's pre-processor decodes the batch (JPEGs on the GPU)."""
-    files = []
-    for row in batch:
-        im = row['image']
-        data = im.get('bytes')
-        if data is None:
-            with open(im['path'], 'rb') as f:
-                data = f.read()
-        files.append(data)
-    return files, torch.as_tensor([row['index'] for row in batch])
+    return [read_encoded(row['image']) for row in batch], torch.as_tensor([row['index'] for row in batch])
+
+
+def encoded_eval_collate(batch):
+    """collate_fn for `EncodedRows` (pigeon_b200.benchmark: rows of a BenchmarkDataset or EvalDataset): reads every
+    view's file of every row, row by row, and stacks the labels.  No CUDA work, so it may run on DataLoader workers;
+    `encoded_pixel_values` turns the batch into pixel_values in the main process."""
+    return {'files': [read_encoded(im) for row in batch for im in row['images']],
+            'views': len(batch[0]['images']), 'square_crop': bool(batch[0]['square_crop']),
+            'labels': torch.as_tensor(np.stack([np.asarray(row['labels']) for row in batch])),
+            'labels_clf': torch.as_tensor(np.asarray([row['labels_clf'] for row in batch]))}
+
+
+def encoded_pixel_values(batch, processor):
+    """A batch of `encoded_eval_collate` -> the model's keyword arguments: pixel_values [B, 3 * views, 336, 336] on
+    the device from one processor call (JPEG decode + pre-processing for the whole batch), labels, labels_clf."""
+    px = processor(images=batch['files'], square_crop=batch['square_crop'])['pixel_values']
+    b = len(batch['files']) // batch['views']
+    return {'pixel_values': px.view(b, 3 * batch['views'], px.shape[2], px.shape[3]),
+            'labels': batch['labels'], 'labels_clf': batch['labels_clf']}
 
 
 def embed_images(loaded_model: Any, dataset, num_workers: int = 0, save_dir: Optional[str] = 'data/landmark_embeddings',

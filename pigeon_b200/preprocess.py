@@ -12,6 +12,8 @@ JPEG parser does not decode) is decoded by Pillow on the host, the reference's o
 either way.  `gpu_decoded` / `host_decoded` count the two routes.  A JPEG with corrupt entropy-coded data raises.
 `jpeg_multiscan=True` sends progressive and multi-scan JPEGs to the GPU decoder as well (opt-in until it is measured at
 least as fast as the host route on progressive photos; DESIGN.md §1).
+`square_crop=True` (a keyword of the call) first cuts every decoded image to its centred square, the reference's
+`BenchmarkDataset._crop_images` (benchmark_dataset.py:52-66): a strided view of a device image, a slice of a host one.
 """
 from __future__ import annotations
 
@@ -41,6 +43,19 @@ def _to_u8_rgb(img) -> np.ndarray:
     return np.ascontiguousarray(img)
 
 
+def square_crop_box(h: int, w: int) -> tuple:
+    """(h0, w0, s) of the centred square crop `image[h0:h0+s, w0:w0+s]`, with the reference's rounding
+    (benchmark_dataset.py:61-64: `int((h - s) / 2)`)."""
+    s = min(h, w)
+    return int((h - s) / 2), int((w - s) / 2), s
+
+
+def _square(img):
+    """Centred square view of an [H, W, 3] array or tensor (rows keep their stride, pixels stay contiguous)."""
+    h0, w0, s = square_crop_box(img.shape[0], img.shape[1])
+    return img[h0:h0 + s, w0:w0 + s]
+
+
 def route_encoded(data, multiscan: bool = False) -> tuple:
     """('gpu', info) for a file the GPU JPEG decoder takes, ('host', info) for one Pillow decodes on the host (PNG,
     progressive JPEG unless `multiscan`, anything else the parser does not decode); ValueError for a JPEG with corrupt
@@ -56,7 +71,8 @@ def route_encoded(data, multiscan: bool = False) -> tuple:
 class ClipImageProcessor:
     """Call-compatible with the way the reference uses `CLIPProcessor` for images: `proc(images=..., return_tensors='pt')`
     returns a dict with 'pixel_values' (here a CUDA tensor).  `dtype=torch.float16` writes the tower's input type directly.
-    `jpeg_multiscan=True` decodes encoded progressive and multi-scan JPEGs on the GPU instead of with Pillow."""
+    `jpeg_multiscan=True` decodes encoded progressive and multi-scan JPEGs on the GPU instead of with Pillow.
+    `proc(images, square_crop=True)` cuts each image to its centred square before the resize (BenchmarkDataset)."""
 
     def __init__(self, size: int = 336, image_mean: Sequence[float] = CLIP_MEAN, image_std: Sequence[float] = CLIP_STD,
                  device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float32,
@@ -96,7 +112,7 @@ class ClipImageProcessor:
                                            int(self.dtype == torch.float16), current_stream_ptr()), "pg_preprocess_clip")
         return out
 
-    def __call__(self, images=None, return_tensors: str = "pt", **kwargs):
+    def __call__(self, images=None, return_tensors: str = "pt", square_crop: bool = False, **kwargs):
         if images is None:
             raise ValueError("You have to specify images.")
         if not isinstance(images, (list, tuple)):
@@ -105,7 +121,7 @@ class ClipImageProcessor:
         gpu_idx, gpu_files, gpu_infos = [], [], []
         for i, img in enumerate(images):
             if isinstance(img, torch.Tensor) and img.is_cuda:
-                dev[i] = img
+                dev[i] = _square(img) if square_crop else img
                 continue
             if isinstance(img, (bytes, bytearray, memoryview)):
                 try:
@@ -120,12 +136,14 @@ class ClipImageProcessor:
                 from PIL import Image
                 img = Image.open(io.BytesIO(bytes(img)))
                 self.host_decoded += 1
-            a = torch.from_numpy(_to_u8_rgb(img))
-            dev[i] = a.pin_memory().to(self.device, non_blocking=True)
+            a = _to_u8_rgb(img)
+            if square_crop:
+                a = np.ascontiguousarray(_square(a))
+            dev[i] = torch.from_numpy(a).pin_memory().to(self.device, non_blocking=True)
         if gpu_files:
             if self._jpeg is None:
                 self._jpeg = jpeg.JpegDecoder(self.device)
             for i, t in zip(gpu_idx, self._jpeg.decode(gpu_files, gpu_infos)):
-                dev[i] = t
+                dev[i] = _square(t) if square_crop else t
             self.gpu_decoded += len(gpu_files)
         return {"pixel_values": self.preprocess_device(dev)}

@@ -2,6 +2,7 @@
 """Entry points of the hot path with the reference's CLI (run.py:21-93): `embed`, `evaluate` and `finetune`.
 
     python run.py evaluate HEAD.model -l DATASET_DIR [-b BASE.model] [--yfcc] [--metrics]
+    python run.py evaluate HEAD.model -l BENCHMARK -b BASE.model [--yfcc] [--metrics] [-w WORKERS]   # config.BENCHMARKS
     python run.py embed CLIP.model -l DATASET_DIR [--jpeg-multiscan]                             # image column + index
     python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading]     # tower + head (run.py:165-169)
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
@@ -17,22 +18,34 @@ reference (run.py:143-162); none are shipped with either repository.
 `--metrics` (evaluate, finetune) evaluates with `metrics.compute_geoguessr_metrics`, as the reference's evaluate.py and
 train_modes.py do: the full GeoGuessr table, with Country_accuracy against config.COUNTRY_PATH.  Without it only
 Geocell_accuracy is computed.
+
+`evaluate -l NAME`, when NAME is not a directory and config.BENCHMARKS exists, evaluates the benchmark NAME listed there (a
+JSON file the user supplies: {name: {"meta": CSV, "images": folder prefix}}) as the reference's run.py:158-162 does, through
+`benchmark.BenchmarkDataset`.  A split whose rows hold encoded `image` columns and no `pixel_values` (the reference's raw
+holdout splits) is wrapped in `benchmark.EvalDataset`.  Both are decoded and pre-processed on the GPU batch by batch.
 """
 import argparse
 import logging
+import os
 
 import torch
 
 from pigeon_b200 import CLIPEmbedding, ProtoRefiner, SuperGuessr
 from pigeon_b200 import config as cfg
-from pigeon_b200.loops import embed_images, encoded_image_collate, evaluate_model
+from pigeon_b200.loops import embed_images, encoded_eval_collate, encoded_image_collate, evaluate_model
 
 logger = logging.getLogger('run')
 
 
 def evaluate(model: str, dataset, yfcc: bool, landmarks: bool = False, base_model: str = None, heading: bool = False,
-             refine: bool = True, metrics=None):
-    """reference evaluation/evaluate.py:10-86."""
+             refine: bool = True, metrics=None, num_workers: int = 0):
+    """reference evaluation/evaluate.py:10-86.  A BenchmarkDataset or EvalDataset is read as encoded files and
+    pre-processed on the GPU batch by batch; the model's `panorama` is the dataset's (the reference always builds
+    panorama=True, which a benchmark's single view cannot take)."""
+    from pigeon_b200.benchmark import BenchmarkDataset, EvalDataset
+    encoded = isinstance(dataset, (BenchmarkDataset, EvalDataset))
+    if encoded and base_model is None:
+        raise ValueError('Evaluating images needs a base model (-b): the prediction head alone takes embeddings, not pixels.')
     embed_model = None
     if base_model is not None:
         from transformers import CLIPVisionModel
@@ -40,7 +53,8 @@ def evaluate(model: str, dataset, yfcc: bool, landmarks: bool = False, base_mode
         if base_model != cfg.CLIP_MODEL:
             from pigeon_b200 import load_state_dict
             load_state_dict(embed_model, torch.load(base_model, map_location='cpu'))       # :37-40
-    full_model = SuperGuessr(embed_model, panorama=True, hierarchical=False, multi_task=False, heading=heading,
+    panorama = dataset.panorama if encoded else True
+    full_model = SuperGuessr(embed_model, panorama=panorama, hierarchical=False, multi_task=False, heading=heading,
                              freeze_base=True, yfcc=yfcc, num_candidates=50)               # :42-44
     full_model.to('cuda')
     # :45-46 — the PIGEOTTO head first, then `model` on top: entries `model` does not carry keep the base head's values
@@ -67,7 +81,11 @@ def evaluate(model: str, dataset, yfcc: bool, landmarks: bool = False, base_mode
             refiner = ProtoRefiner(40, False, 100000, proto_path=proto_path, dataset_path=dataset_path, protos=protos,
                                    temperature=0.6, verbose=False)
         print(refiner)
-    return evaluate_model(full_model, dataset, metrics, None, refiner)
+    if encoded:
+        from pigeon_b200.preprocess import ClipImageProcessor
+        return evaluate_model(full_model, dataset.encoded(), metrics, None, refiner, num_workers=num_workers,
+                              collate_fn=encoded_eval_collate, processor=ClipImageProcessor())
+    return evaluate_model(full_model, dataset, metrics, None, refiner, num_workers=num_workers)
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -85,6 +103,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
     p.add_argument('--jpeg-multiscan', action='store_true',
                    help='embed: decode progressive and multi-scan JPEGs on the GPU too (by default Pillow decodes them)')
+    p.add_argument('-w', '--workers', type=int, default=0,
+                   help='evaluate: DataLoader worker processes (they read the image files of a benchmark or raw split)')
     p.add_argument('--metrics', action='store_true',
                    help='evaluate / finetune: report compute_geoguessr_metrics (needs config.COUNTRY_PATH)')
     return p
@@ -102,8 +122,14 @@ def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.load is None:
         raise NotImplementedError('A dataset must be given with -l (the reference regenerates it from un-shipped raw data).')
+    load = args.load.split(',')[0]
+    if args.mode == 'evaluate' and not os.path.isdir(load) and os.path.isfile(cfg.BENCHMARKS):   # run.py:158-162
+        from pigeon_b200.benchmark import BenchmarkDataset
+        print(evaluate(args.name, BenchmarkDataset(load), args.yfcc, args.landmarks, base_model=args.base,
+                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args), num_workers=args.workers))
+        return
     from datasets import DatasetDict
-    dataset = DatasetDict.load_from_disk(args.load.split(',')[0])
+    dataset = DatasetDict.load_from_disk(load)
     if args.mode == 'pretrain':
         from pigeon_b200.training import pretrain
         pretrain(args.name, dataset.with_format('torch'), cfg.PRETAIN_ARGS_YFCC if args.yfcc else cfg.PRETAIN_ARGS,
@@ -130,8 +156,13 @@ def main(argv=None):
         embed_images(model, splits, collate_fn=encoded_image_collate)
     else:
         split = dataset['test'] if 'test' in dataset else dataset[list(dataset.keys())[-1]]
-        print(evaluate(args.name, split.with_format('torch'), args.yfcc, args.landmarks, base_model=args.base,
-                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args)))
+        split = split.with_format('torch')
+        columns = getattr(split, 'column_names', None) or ()
+        if 'image' in columns and 'pixel_values' not in columns:                               # raw holdout split
+            from pigeon_b200.benchmark import EvalDataset
+            split = EvalDataset(split)
+        print(evaluate(args.name, split, args.yfcc, args.landmarks, base_model=args.base,
+                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args), num_workers=args.workers))
 
 
 if __name__ == '__main__':
