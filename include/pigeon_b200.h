@@ -264,11 +264,29 @@ size_t pg_jpeg_workspace_bytes(const pg_jpeg_info* infos_host, int32_t n, int64_
  * host-to-device copy of offsets_host[n] bytes; pinned memory makes it asynchronous), infos_host[i] its pg_jpeg_parse
  * or pg_jpeg_parse_multiscan result, dst_host[i] a descriptor of its height x width x 3 uint8 RGB destination
  * (written; the same descriptors feed pg_preprocess_clip).  status_out: device i32 [n], the parse status of a skipped
- * file, else PG_JPEG_OK or the entropy-data error of that file (whose destination is then left unwritten).  Three
- * launches for a batch of single-scan files.  A batch with multi-scan files also zeroes their coefficients and decodes
- * their scans in one launch per dependency level (pg_jpeg_scan.level), all in stream order. */
+ * file, else PG_JPEG_OK or the entropy-data error of that file (whose destination is then left unwritten).  A batch of
+ * single-scan files takes three or four launches: the Huffman decode of short entropy-coded segments (restart
+ * intervals, small files) with one thread each and of long ones (a photo without restart markers) with one CTA each,
+ * chunked and self-synchronising, then the IDCT and the colour conversion.  A batch with multi-scan files also zeroes
+ * their coefficients and decodes their scans in one launch per dependency level (pg_jpeg_scan.level), all in stream
+ * order. */
 int pg_jpeg_decode(const uint8_t* packed_host, const int64_t* offsets_host, const pg_jpeg_info* infos_host, int32_t n,
                    const pg_image* dst_host, void* workspace, size_t workspace_bytes, int32_t* status_out, void* stream);
+/* Huffman decode of single-scan segments in pg_jpeg_decode, process-wide: 0 = automatic (default; segments of at least
+ * 32768 compressed bytes take the chunked kernel, shorter ones one thread each), 1 = one thread per segment, 2 = the
+ * chunked kernel for every segment.  chunk_bytes > 0 forces the chunk size in de-stuffed bytes (raised where a segment
+ * would need more than 1024 chunks); 0 sizes chunks automatically.  All give the same bytes and statuses; the switch
+ * exists for tests and A/B benchmarks, not for tuning.  Returns 1 for a mode outside {0, 1, 2} or chunk_bytes < 0. */
+int pg_jpeg_set_schedule(int32_t mode, int32_t chunk_bytes);
+/* Host-only test entry: the entropy decode of pg_jpeg_decode on the CPU, for single-scan files (a multi-scan info is an
+ * error).  chunk_bytes = 0 runs the one-thread-per-segment decoder; > 0 runs the chunked decoder's functions, in its
+ * order of rounds, at that chunk size; < 0 at the automatic size.  coef_out (NULL: not returned) receives the int16
+ * blocks, 64 in natural order each, of every image with an OK info in batch order, its components in order, each
+ * component's grid padded to whole MCUs row by row; blocks of a failed image are unspecified.  status_out[n] as
+ * pg_jpeg_decode's; rounds_out[n] (optional) the most synchronisation rounds any segment of the image took (0 for the
+ * one-thread decoder).  Returns the number of blocks, or -1 (pg_last_error() names the reason). */
+int64_t pg_jpeg_entropy_host(const uint8_t* packed_host, const int64_t* offsets_host, const pg_jpeg_info* infos_host,
+                             int32_t n, int32_t chunk_bytes, int16_t* coef_out, int32_t* status_out, int32_t* rounds_out);
 
 /* ---------------------------------------------------------------------------------------------------
  * Fine-tune step, head-only part ("next" row N1 with a frozen or absent base model): what loss.backward() and

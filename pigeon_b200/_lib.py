@@ -181,6 +181,9 @@ SIGNATURES = {
     "pg_jpeg_workspace_bytes": (c_size_t, [C.POINTER(JpegInfo), c_int32, c_int64]),
     "pg_jpeg_decode": (c_int32, [c_void_p, c_void_p, C.POINTER(JpegInfo), c_int32, c_void_p, c_void_p, c_size_t, c_void_p,
                                  c_void_p]),
+    "pg_jpeg_set_schedule": (c_int32, [c_int32, c_int32]),
+    "pg_jpeg_entropy_host": (c_int64, [c_void_p, c_void_p, C.POINTER(JpegInfo), c_int32, c_int32, c_void_p, c_void_p,
+                                       c_void_p]),
     "pg_head_loss_grad": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_double,
                                     c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pg_head_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,

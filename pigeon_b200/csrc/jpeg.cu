@@ -1,8 +1,10 @@
 // Baseline JPEG decoding on the GPU, byte-identical to Pillow's `Image.open(f).convert('RGB')` over libjpeg-turbo with
 // its defaults (ISLOW IDCT, fancy upsampling).  Four stages:
 //   host   marker walk (pg_jpeg_parse): frame, tables, restart interval, entropy-coded byte range, restart segments;
-//   kernel 1  Huffman decode, one thread per entropy-coded segment (a restart interval, or the whole scan without DRI):
-//             byte de-stuffing, DC prediction reset per segment, quantised coefficients -> int16 blocks;
+//   kernel 1  Huffman decode of each entropy-coded segment (a restart interval, or the whole scan without DRI): byte
+//             de-stuffing, DC prediction reset per segment, quantised coefficients -> int16 blocks.  A short segment
+//             takes one thread (entropy_kernel); a long one, such as a photo without restart markers, one CTA that
+//             decodes it in self-synchronising chunks (chunked_kernel); both kernels may run in one call;
 //   kernel 2  dequantise + jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2, 64-bit products like libjpeg's JLONG) + the
 //             post-IDCT range-limit table with its `& RANGE_MASK` wrap -> component planes padded to whole MCUs;
 //   kernel 3  fancy upsampling (jdsample.c h2v1 / h2v2, plain replication when the chroma width is <= 2) fused with
@@ -19,6 +21,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
+#include <climits>
 #include <map>
 #include <string>
 #include <vector>
@@ -603,7 +607,8 @@ struct BitReader {
   __host__ __device__ __forceinline__ bool overrun() const { return zeros * 8 > nbits; }
 };
 
-__host__ __device__ __forceinline__ int huff_decode(BitReader& br, const HuffTbl& t) {
+template <class Reader>
+__host__ __device__ __forceinline__ int huff_decode(Reader& br, const HuffTbl& t) {
   const int e = t.look[br.acc >> (64 - LOOK_BITS)];
   if (e >> 8) {
     br.acc <<= (e >> 8);
@@ -693,6 +698,401 @@ entropy_kernel(const uint8_t* __restrict__ bytes, const ImgDesc* __restrict__ im
   const ImgDesc& im = imgs[sg.img];
   const int err = decode_segment(bytes, im, tbls, sg, blk_smem[lane], coef);
   if (err) atomicCAS(status + im.orig, 0, err);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Device: chunked entropy decode of long single-scan segments (self-synchronising Huffman decoding)
+// ------------------------------------------------------------------------------------------------------------------
+//
+// After Weissenberger and Schmidt, "Massively parallel Huffman decoding on GPUs" (ICPP 2018).  One CTA per segment:
+//   1. de-stuff the segment (FF 00 -> FF, fill bytes dropped) into plain bytes, so that a chunk can start at any bit;
+//   2. cut those bytes into chunks.  A chunk owns the blocks whose DC code starts inside it; its state at a block start
+//      is (bit offset, block slot within the MCU), and its exit state is the state at the first block start at or after
+//      its end.  Round 0 decodes every chunk from a guess (its first bit, slot 0; chunk 0 from the true state); each
+//      later round re-decodes the chunks whose start (the previous chunk's exit) changed, until none did.  Huffman codes
+//      resynchronise within a few codes, so that takes few rounds; it never takes more than one round per chunk;
+//   3. block-wide exclusive scans of the blocks each chunk starts and of its DC differences per component give every
+//      chunk its absolute first block and DC predictors; every chunk decodes once more and writes its blocks.
+// Only that last pass reports errors: the first event in stream order that decode_segment meets, a bad code at its
+// block or an overrun at the end of its MCU.  A speculative decode that meets a bad code reports nothing (chunk_sync).
+// All synchronisation is __syncthreads within the CTA.
+
+constexpr int CHUNK_THREADS = 256;
+constexpr int MIN_CHUNK_BYTES = 512;    // automatic chunk size: max(MIN_CHUNK_BYTES, de-stuffed bytes / CHUNK_THREADS)
+constexpr int MAX_CHUNKS = 1024;        // chunk states live in shared memory; a forced size is raised to fit them
+constexpr long long NO_EVENT = LLONG_MAX;
+
+// Segments of at least this many compressed bytes take the chunked kernel under the automatic schedule.
+constexpr long long LONG_SEGMENT_BYTES = 32768;
+
+// Process-wide entropy-kernel choice (pg_jpeg_set_schedule): 0 = automatic, 1 = one thread per segment, 2 = chunked
+// for every single-scan segment; a nonzero chunk size forces the chunks' size in bytes.
+std::atomic<int> g_jpeg_schedule{0};
+std::atomic<int> g_jpeg_chunk_bytes{0};
+
+// jdhuff.c's de-stuffing as BitReader::fill applies it: after an FF, further FF fill bytes and one 00 are dropped.  A
+// segment holds no marker (walk_scan ends it at the first FF of one), so every FF is followed by FF or 00.
+__host__ __device__ __forceinline__ bool stuffing_byte(const uint8_t* d, long long i) {
+  return i > 0 && d[i - 1] == 0xFF && (d[i] == 0xFF || d[i] == 0x00);
+}
+
+__host__ __device__ inline long long destuff_count(const uint8_t* d, long long i0, long long i1) {
+  long long n = 0;
+  for (long long i = i0; i < i1; ++i) n += !stuffing_byte(d, i);
+  return n;
+}
+
+__host__ __device__ inline void destuff_copy(const uint8_t* d, long long i0, long long i1, uint8_t* out) {
+  for (long long i = i0; i < i1; ++i)
+    if (!stuffing_byte(d, i)) *out++ = d[i];
+}
+
+// Chunk size in bytes and chunk count of a segment of `len` de-stuffed bytes; `forced` > 0 is the forced size.
+__host__ __device__ inline void chunk_geometry(long long len, int forced, long long* cb, int* nch) {
+  long long c = forced > 0 ? forced : std::max<long long>(MIN_CHUNK_BYTES, (len + CHUNK_THREADS - 1) / CHUNK_THREADS);
+  if ((len + c - 1) / c > MAX_CHUNKS) c = (len + MAX_CHUNKS - 1) / MAX_CHUNKS;
+  *cb = c;
+  *nch = (int)std::max<long long>(1, (len + c - 1) / c);
+}
+
+// BitReader over de-stuffed bytes, started at any bit; zero bytes past the end, as BitReader feeds them.
+struct PlainBits {
+  const uint8_t* p;
+  const uint8_t* end;
+  uint64_t acc;
+  int nbits;
+  int err;
+  long long past;                    // zero bytes fed past the end
+
+  __host__ __device__ __forceinline__ void start(const uint8_t* data, long long len, long long bit) {
+    const long long byte = bit >> 3;
+    p = data + std::min(byte, len);
+    end = data + len;
+    past = byte > len ? byte - len : 0;
+    acc = 0;
+    nbits = 0;
+    err = 0;
+    fill();
+    acc <<= (bit & 7);
+    nbits -= (int)(bit & 7);
+  }
+  __host__ __device__ __forceinline__ void fill() {
+    while (nbits <= 56) {
+      uint32_t c = 0;
+      if (p < end) c = *p++; else ++past;
+      acc |= (uint64_t)c << (56 - nbits);
+      nbits += 8;
+    }
+  }
+  __host__ __device__ __forceinline__ int get(int s) {
+    const int r = (int)(acc >> (64 - s));
+    acc <<= s;
+    nbits -= s;
+    return r;
+  }
+  __host__ __device__ __forceinline__ long long bit(const uint8_t* data) const { return ((p - data) + past) * 8 - nbits; }
+};
+
+// One segment as its chunks see it: the de-stuffed bytes, the MCU's block slots and where each slot's blocks go.
+struct ChunkSeg {
+  const uint8_t* data;
+  long long len;                     // de-stuffed bytes
+  const HuffTbl* tb;                 // DC and AC table of component c at tb[2c], tb[2c + 1]
+  int bpm, total, mcu0, mcux;        // blocks per MCU, blocks of the segment, its first MCU, MCUs per row
+  int comp[6];                       // component of each slot
+  long long off[6];                  // first block of the slot's component + its offset within the MCU
+  int rowstep[6], colstep[6];        // blocks per MCU row (v * bw) and per MCU column (h) of the slot's component
+};
+
+__host__ __device__ inline void chunk_seg_init(ChunkSeg& cs, const ImgDesc& im, const Seg& sg, const uint8_t* data,
+                                               long long len, const HuffTbl* tb) {
+  cs.data = data;
+  cs.len = len;
+  cs.tb = tb;
+  cs.mcu0 = sg.mcu0;
+  cs.mcux = im.mcux;
+  int s = 0;
+  for (int c = 0; c < im.ncomp; ++c)
+    for (int bv = 0; bv < im.c[c].v; ++bv)
+      for (int bh = 0; bh < im.c[c].h; ++bh, ++s) {
+        cs.comp[s] = c;
+        cs.off[s] = im.c[c].coef_off + (long long)bv * im.c[c].bw + bh;
+        cs.rowstep[s] = im.c[c].v * im.c[c].bw;
+        cs.colstep[s] = im.c[c].h;
+      }
+  cs.bpm = s;
+  cs.total = sg.nmcu * s;
+}
+
+// One block, as decode_segment decodes it; with STORE its AC coefficients go to `blk` (zeroed first).  Returns true on a
+// bad code, where decode_segment stops without storing the block.
+template <bool STORE>
+__host__ __device__ __forceinline__ bool chunk_block(PlainBits& br, const HuffTbl& dct, const HuffTbl& act, int16_t* blk,
+                                                     int* diff) {
+#ifdef __CUDA_ARCH__
+  const uint8_t* natural = c_natural;
+#else
+  const uint8_t* natural = h_natural;
+#endif
+  br.fill();
+  int s = huff_decode(br, dct);
+  if (br.err) return true;
+  if (s) s = huff_extend(br.get(s), s);
+  *diff = s;
+  if (STORE)
+    for (int i = 0; i < 64; i += 8) *reinterpret_cast<uint4*>(blk + i) = make_uint4(0, 0, 0, 0);
+  for (int k = 1; k < 64;) {
+    if (br.nbits < 32) br.fill();
+    const int rs = huff_decode(br, act);
+    if (br.err) return true;
+    const int r = rs >> 4;
+    s = rs & 15;
+    if (s) {
+      k += r;
+      if (k > 63) return true;
+      const int v = br.get(s);
+      if (STORE) blk[natural[k]] = (int16_t)huff_extend(v, s);
+      ++k;
+    } else {
+      if (r != 15) break;
+      k += 16;
+    }
+  }
+  return false;
+}
+
+struct ChunkRun {
+  long long exit;                    // (bit << 3) | slot
+  int count;                         // blocks started
+  unsigned dc0, dc1, dc2;            // DC differences per component, modulo 2^32 like decode_segment's int predictor
+};
+
+// Synchronisation pass: decodes the blocks that start in [state's bit, end_bit) without writing them.  A bad code means
+// the decode started out of step: it resumes one bit further on, at the same slot, which keeps it resynchronising.  A
+// decode from the true state meets one only where decode_segment stops with the image's error; nothing after that
+// point is written or reported, so what the pass counts there does not matter.
+__host__ __device__ inline ChunkRun chunk_sync(const ChunkSeg& cs, long long state, long long end_bit) {
+  ChunkRun r{0, 0, 0u, 0u, 0u};
+  long long bit = state >> 3;
+  int slot = (int)(state & 7);
+  PlainBits br;
+  br.start(cs.data, cs.len, bit);
+  while (bit < end_bit) {
+    const int c = cs.comp[slot];
+    int diff = 0;
+    if (chunk_block<false>(br, cs.tb[2 * c], cs.tb[2 * c + 1], nullptr, &diff)) {
+      bit = br.bit(cs.data) + 1;
+      br.start(cs.data, cs.len, bit);
+      continue;
+    }
+    if (c == 0) r.dc0 += diff; else if (c == 1) r.dc1 += diff; else r.dc2 += diff;
+    ++r.count;
+    slot = slot + 1 == cs.bpm ? 0 : slot + 1;
+    bit = br.bit(cs.data);
+  }
+  r.exit = (bit << 3) | slot;
+  return r;
+}
+
+// Final pass of one synchronised chunk: block `block` of the segment onwards, with DC predictors p0..p2, written to
+// `coef` through `blk` (64 int16 of scratch).  Returns the chunk's first event, 2 * block for a bad code and
+// 2 * (last block of the MCU) + 1 for an MCU that ends past the data, or NO_EVENT.
+__host__ __device__ inline long long chunk_final(const ChunkSeg& cs, long long state, long long end_bit, long long block,
+                                                 unsigned p0, unsigned p1, unsigned p2, int16_t* blk,
+                                                 int16_t* __restrict__ coef) {
+  long long bit = state >> 3;
+  int slot = (int)(state & 7);
+  PlainBits br;
+  br.start(cs.data, cs.len, bit);
+  const long long data_bits = cs.len * 8;
+  while (block < cs.total && bit < end_bit) {
+    const int c = cs.comp[slot];
+    int diff = 0;
+    if (chunk_block<true>(br, cs.tb[2 * c], cs.tb[2 * c + 1], blk, &diff)) return 2 * block;
+    unsigned pred;
+    if (c == 0) pred = p0 += diff; else if (c == 1) pred = p1 += diff; else pred = p2 += diff;
+    blk[0] = (int16_t)pred;
+    const int mcu = cs.mcu0 + (int)(block / cs.bpm);
+    const int my = mcu / cs.mcux, mx = mcu - my * cs.mcux;
+    const long long b = cs.off[slot] + (long long)my * cs.rowstep[slot] + (long long)mx * cs.colstep[slot];
+    uint4* o = reinterpret_cast<uint4*>(coef + b * 64);
+    for (int i = 0; i < 8; ++i) o[i] = reinterpret_cast<const uint4*>(blk)[i];
+    bit = br.bit(cs.data);
+    if (slot == cs.bpm - 1 && bit > data_bits) return 2 * block + 1;
+    ++block;
+    slot = slot + 1 == cs.bpm ? 0 : slot + 1;
+  }
+  return NO_EVENT;
+}
+
+struct ChunkSums {
+  long long n;
+  unsigned a, b, c;
+};
+
+__device__ __forceinline__ ChunkSums operator+(const ChunkSums& x, const ChunkSums& y) {
+  return ChunkSums{x.n + y.n, x.a + y.a, x.b + y.b, x.c + y.c};
+}
+
+// Exclusive scan over the CTA's threads in thread order; *total gets the sum.  `ws` holds one value per warp.
+__device__ __forceinline__ ChunkSums block_exclusive_scan(ChunkSums v, ChunkSums* ws, ChunkSums* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+  ChunkSums inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    ChunkSums y{__shfl_up_sync(0xffffffffu, inc.n, o), __shfl_up_sync(0xffffffffu, inc.a, o),
+                __shfl_up_sync(0xffffffffu, inc.b, o), __shfl_up_sync(0xffffffffu, inc.c, o)};
+    if (lane >= o) inc = inc + y;
+  }
+  if (lane == 31) ws[warp] = inc;
+  __syncthreads();
+  ChunkSums before{0, 0u, 0u, 0u}, all{0, 0u, 0u, 0u};
+  for (int w = 0; w < nwarp; ++w) {
+    if (w < warp) before = before + ws[w];
+    all = all + ws[w];
+  }
+  __syncthreads();
+  *total = all;
+  ChunkSums ex{inc.n - v.n, inc.a - v.a, inc.b - v.b, inc.c - v.c};
+  return before + ex;
+}
+
+// One CTA per long segment.  Dynamic shared memory: the chunk states, `cap` chunks (>= every segment's chunk count).
+__global__ void __launch_bounds__(CHUNK_THREADS, 2)
+chunked_kernel(const uint8_t* __restrict__ bytes, const ImgDesc* __restrict__ imgs, const HuffTbl* __restrict__ tbls,
+               const Seg* __restrict__ segs, int cap, int forced, uint8_t* destuffed, int16_t* __restrict__ coef,
+               int* __restrict__ status) {
+  __shared__ __align__(16) HuffTbl tb[6];
+  __shared__ __align__(16) int16_t blk_smem[CHUNK_THREADS][64];
+  __shared__ ChunkSeg cs;
+  __shared__ ChunkSums scan_ws[CHUNK_THREADS / 32];
+  __shared__ unsigned long long first_event;
+  extern __shared__ __align__(16) unsigned char chunk_smem[];
+  long long* st = reinterpret_cast<long long*>(chunk_smem);        // start state of each chunk
+  long long* ex = st + cap;                                        // its exit state
+  int* cnt = reinterpret_cast<int*>(ex + cap);                      // blocks it starts
+  unsigned* d0 = reinterpret_cast<unsigned*>(cnt + cap);            // its DC differences per component
+  unsigned* d1 = d0 + cap;
+  unsigned* d2 = d1 + cap;
+
+  const int tid = threadIdx.x, T = blockDim.x;
+  const Seg sg = segs[blockIdx.x];
+  const ImgDesc& im = imgs[sg.img];
+  constexpr int TBL_WORDS = sizeof(HuffTbl) / 4;
+  for (int w = tid; w < 2 * im.ncomp * TBL_WORDS; w += T) {
+    const int t = w / TBL_WORDS, j = w - t * TBL_WORDS;
+    const HuffTbl& src = tbls[(t & 1) ? im.c[t >> 1].ac : im.c[t >> 1].dc];
+    reinterpret_cast<uint32_t*>(&tb[t])[j] = reinterpret_cast<const uint32_t*>(&src)[j];
+  }
+
+  // 1. de-stuff: each thread a contiguous byte range, placed by a scan of the data-byte counts
+  const long long n = sg.end - sg.start;
+  const uint8_t* src = bytes + sg.start;
+  uint8_t* dst = destuffed + sg.start;
+  const long long per = (n + T - 1) / T;
+  const long long i0 = std::min(n, tid * per), i1 = std::min(n, i0 + per);
+  ChunkSums tot;
+  const ChunkSums at = block_exclusive_scan(ChunkSums{destuff_count(src, i0, i1), 0u, 0u, 0u}, scan_ws, &tot);
+  destuff_copy(src, i0, i1, dst + at.n);
+  if (tid == 0) {
+    chunk_seg_init(cs, im, sg, dst, tot.n, tb);
+    first_event = (unsigned long long)NO_EVENT;
+  }
+  __syncthreads();                   // de-stuffed bytes (global) and cs visible to the CTA
+
+  // 2. synchronisation rounds; thread tid owns chunks [c0, c1)
+  long long cb;
+  int nch;
+  chunk_geometry(cs.len, forced, &cb, &nch);
+  const int per_thread = (nch + T - 1) / T;
+  const int c0 = std::min(nch, tid * per_thread), c1 = std::min(nch, c0 + per_thread);
+  unsigned dirty = 0;
+  for (int t = c0; t < c1; ++t) {
+    st[t] = (t * cb * 8) << 3;
+    ChunkRun r{0, 0, 0u, 0u, 0u};
+    if (t < nch - 1) r = chunk_sync(cs, st[t], (t + 1) * cb * 8);
+    ex[t] = r.exit; cnt[t] = r.count; d0[t] = r.dc0; d1[t] = r.dc1; d2[t] = r.dc2;
+  }
+  for (;;) {
+    __syncthreads();
+    for (int t = std::max(c0, 1); t < c1; ++t)
+      if (ex[t - 1] != st[t]) {
+        st[t] = ex[t - 1];
+        dirty |= 1u << (t - c0);
+      }
+    if (!__syncthreads_or(dirty != 0)) break;
+    for (int t = c0; t < c1; ++t)
+      if (dirty & (1u << (t - c0))) {
+        if (t < nch - 1) {
+          const ChunkRun r = chunk_sync(cs, st[t], (t + 1) * cb * 8);
+          ex[t] = r.exit; cnt[t] = r.count; d0[t] = r.dc0; d1[t] = r.dc1; d2[t] = r.dc2;
+        }
+      }
+    dirty = 0;
+  }
+
+  // 3. absolute first block and DC predictors of every chunk, then the final pass
+  ChunkSums mine{0, 0u, 0u, 0u};
+  for (int t = c0; t < c1; ++t) mine = mine + ChunkSums{cnt[t], d0[t], d1[t], d2[t]};
+  ChunkSums pre = block_exclusive_scan(mine, scan_ws, &tot);
+  long long event = NO_EVENT;
+  for (int t = c0; t < c1; ++t) {
+    const long long end_bit = t == nch - 1 ? LLONG_MAX : (t + 1) * cb * 8;
+    event = std::min(event, chunk_final(cs, st[t], end_bit, pre.n, pre.a, pre.b, pre.c, blk_smem[tid], coef));
+    pre = pre + ChunkSums{cnt[t], d0[t], d1[t], d2[t]};
+  }
+  if (event != NO_EVENT) atomicMin(&first_event, (unsigned long long)event);
+  __syncthreads();
+  if (tid == 0 && first_event != (unsigned long long)NO_EVENT)
+    atomicCAS(status + im.orig, 0, (first_event & 1) ? ST_OVERRUN : ST_BAD_CODE);
+}
+
+// The chunked decode of one segment on the host, in the kernel's order of rounds and passes.  Returns the segment's
+// error (0 when none) and sets *rounds to the synchronisation rounds it took.
+int chunked_segment_host(const uint8_t* bytes, const ImgDesc& im, const HuffTbl* tbls, const Seg& sg, int forced,
+                         int16_t* coef, int* rounds) {
+  const long long n = sg.end - sg.start;
+  std::vector<uint8_t> buf((size_t)n);
+  destuff_copy(bytes + sg.start, 0, n, buf.data());
+  HuffTbl tb[6];
+  for (int c = 0; c < im.ncomp; ++c) {
+    tb[2 * c] = tbls[im.c[c].dc];
+    tb[2 * c + 1] = tbls[im.c[c].ac];
+  }
+  ChunkSeg cs;
+  chunk_seg_init(cs, im, sg, buf.data(), destuff_count(bytes + sg.start, 0, n), tb);
+  long long cb;
+  int nch;
+  chunk_geometry(cs.len, forced, &cb, &nch);
+  std::vector<long long> st(nch);
+  std::vector<ChunkRun> run(nch, ChunkRun{0, 0, 0u, 0u, 0u});
+  for (int t = 0; t < nch; ++t) {
+    st[t] = (t * cb * 8) << 3;
+    if (t < nch - 1) run[t] = chunk_sync(cs, st[t], (t + 1) * cb * 8);
+  }
+  *rounds = 1;
+  for (;;) {
+    std::vector<int> dirty;
+    for (int t = 1; t < nch; ++t)
+      if (run[t - 1].exit != st[t]) {
+        st[t] = run[t - 1].exit;
+        dirty.push_back(t);
+      }
+    if (dirty.empty()) break;
+    ++*rounds;
+    for (int t : dirty)
+      if (t < nch - 1) run[t] = chunk_sync(cs, st[t], (t + 1) * cb * 8);
+  }
+  long long block = 0, event = NO_EVENT;
+  unsigned p0 = 0, p1 = 0, p2 = 0;
+  alignas(16) int16_t blk[64];
+  for (int t = 0; t < nch; ++t) {
+    const long long end_bit = t == nch - 1 ? LLONG_MAX : (t + 1) * cb * 8;
+    event = std::min(event, chunk_final(cs, st[t], end_bit, block, p0, p1, p2, blk, coef));
+    block += run[t].count;
+    p0 += run[t].dc0; p1 += run[t].dc1; p2 += run[t].dc2;
+  }
+  return event == NO_EVENT ? 0 : (event & 1) ? ST_OVERRUN : ST_BAD_CODE;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1036,7 +1436,7 @@ struct Plan {
   long long multi_coef0 = -1, multi_coef1 = -1;       // blocks [multi_coef0, multi_coef1) hold every multi-scan image
   size_t off_imgs = 0, off_tbls = 0, off_segs = 0, off_planes = 0, off_pix0 = 0, off_scans = 0, off_msegs = 0,
          meta_bytes = 0;
-  size_t off_bytes = 0, off_meta = 0, off_coef = 0, off_plane = 0, total = 0;
+  size_t off_bytes = 0, off_meta = 0, off_coef = 0, off_plane = 0, off_destuff = 0, total = 0;
 };
 
 // Index of the Huffman table (bits, vals) in the batch's de-duplicated table array; -1 for an invalid table.
@@ -1228,6 +1628,7 @@ int make_plan(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info*
   P->off_meta = total; total += P->meta_bytes;
   P->off_coef = total; total += align_up((size_t)P->nblocks * 128, 256);
   P->off_plane = total; total += align_up((size_t)P->plane_bytes, 256);
+  P->off_destuff = total; total += align_up((size_t)packed_bytes, 256);   // de-stuffed long segments, in place
   P->total = total;
   if (!packed) return 0;
   // restart segments, found again by the same walk that validated them in pg_jpeg_parse
@@ -1319,6 +1720,52 @@ int jpeg_scans(const uint8_t* data, int64_t bytes, pg_jpeg_scan* out, int cap) {
   return (int)scans.size();
 }
 
+int jpeg_set_schedule(int mode, int chunk_bytes) {
+  if (mode < 0 || mode > 2 || chunk_bytes < 0) {
+    set_last_error("pg_jpeg_set_schedule: mode %d not in {0, 1, 2} or chunk_bytes %d < 0", mode, chunk_bytes);
+    return 1;
+  }
+  g_jpeg_schedule.store(mode, std::memory_order_relaxed);
+  g_jpeg_chunk_bytes.store(chunk_bytes, std::memory_order_relaxed);
+  return 0;
+}
+
+int64_t jpeg_entropy_host(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_info* infos, int n, int chunk_bytes,
+                          int16_t* coef_out, int32_t* status_out, int32_t* rounds_out) {
+  if (!packed || !offsets || !infos || !status_out || n <= 0) {
+    set_last_error("pg_jpeg_entropy_host: null argument");
+    return -1;
+  }
+  for (int i = 0; i < n; ++i)
+    if (infos[i].status == PG_JPEG_OK && (infos[i].table_mask & PG_JPEG_MULTISCAN)) {
+      set_last_error("pg_jpeg_entropy_host: image %d is a multi-scan file", i);
+      return -1;
+    }
+  Plan P;
+  if (make_plan(packed, offsets, infos, n, offsets[n], nullptr, &P)) return -1;
+  std::vector<int16_t> own;
+  int16_t* coef = coef_out;
+  if (!coef) {
+    own.resize((size_t)P.nblocks * 64);
+    coef = own.data();
+  }
+  memset(coef, 0, (size_t)P.nblocks * 128);
+  for (int i = 0; i < n; ++i) {
+    status_out[i] = infos[i].status;
+    if (rounds_out) rounds_out[i] = 0;
+  }
+  alignas(16) int16_t blk[64];
+  for (const Seg& sg : P.segs) {
+    const ImgDesc& im = P.imgs[sg.img];
+    int err = 0, rounds = 0;
+    if (chunk_bytes == 0) err = decode_segment(packed, im, P.tbls.data(), sg, blk, coef);
+    else err = chunked_segment_host(packed, im, P.tbls.data(), sg, std::max(chunk_bytes, 0), coef, &rounds);
+    if (err && !status_out[im.orig]) status_out[im.orig] = err;
+    if (rounds_out) rounds_out[im.orig] = std::max(rounds_out[im.orig], rounds);
+  }
+  return P.nblocks;
+}
+
 size_t jpeg_workspace_bytes(const pg_jpeg_info* infos, int n, int64_t packed_bytes) {
   Plan P;
   if (make_plan(nullptr, nullptr, infos, n, packed_bytes, nullptr, &P)) return 0;
@@ -1333,6 +1780,13 @@ int jpeg_decode(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_inf
   }
   Plan P;
   if (make_plan(packed, offsets, infos, n, offsets[n], dst, &P)) return 1;
+  // short segments (restart intervals, small files) first, one thread each; then the long ones, one CTA each
+  const int schedule = g_jpeg_schedule.load(std::memory_order_relaxed);
+  const int forced = g_jpeg_chunk_bytes.load(std::memory_order_relaxed);
+  const int nshort = (int)(std::stable_partition(P.segs.begin(), P.segs.end(), [schedule](const Seg& s) {
+                             return schedule == 1 || (schedule == 0 && s.end - s.start < LONG_SEGMENT_BYTES);
+                           }) - P.segs.begin());
+  const int nlong = (int)P.segs.size() - nshort;
   if (!workspace || workspace_bytes < P.total || (reinterpret_cast<uintptr_t>(workspace) & 255)) {
     set_last_error("pg_jpeg_decode: workspace too small (%zu < %zu) or not 256-byte aligned", workspace_bytes, P.total);
     return 1;
@@ -1364,7 +1818,6 @@ int jpeg_decode(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_inf
   const long long* d_pix0 = reinterpret_cast<const long long*>(meta_d + P.off_pix0);
   int16_t* d_coef = reinterpret_cast<int16_t*>(ws + P.off_coef);
   uint8_t* d_planes = ws + P.off_plane;
-  const int nseg = (int)P.segs.size();
   int sms = 132;
   {
     int dev = 0;
@@ -1380,11 +1833,20 @@ int jpeg_decode(const uint8_t* packed, const int64_t* offsets, const pg_jpeg_inf
     e = cudaMemsetAsync(d_coef + P.multi_coef0 * 64, 0, (size_t)(P.multi_coef1 - P.multi_coef0) * 128, stream);
     if (e != cudaSuccess) { set_last_error("pg_jpeg_decode: memset: %s", cudaGetErrorString(e)); return 1; }
   }
-  if (nseg > 0) {
-    const int lanes = lanes_for(nseg);
+  if (nshort > 0) {
+    const int lanes = lanes_for(nshort);
     ProfScope prof("jpeg_entropy", stream);
-    entropy_kernel<<<(nseg + lanes - 1) / lanes, ENTROPY_THREADS, 0, stream>>>(ws + P.off_bytes, d_imgs, d_tbls, d_segs,
-                                                                                nseg, lanes, d_coef, status_out);
+    entropy_kernel<<<(nshort + lanes - 1) / lanes, ENTROPY_THREADS, 0, stream>>>(ws + P.off_bytes, d_imgs, d_tbls, d_segs,
+                                                                                  nshort, lanes, d_coef, status_out);
+  }
+  if (nlong > 0) {
+    const int cap = forced > 0 ? MAX_CHUNKS : CHUNK_THREADS;     // chunk_geometry's bound on a segment's chunks
+    const size_t smem = (size_t)cap * (2 * sizeof(long long) + sizeof(int) + 3 * sizeof(unsigned));
+    e = cudaFuncSetAttribute(chunked_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_last_error("pg_jpeg_decode: %s", cudaGetErrorString(e)); return 1; }
+    ProfScope prof("jpeg_entropy_chunked", stream);
+    chunked_kernel<<<nlong, CHUNK_THREADS, smem, stream>>>(ws + P.off_bytes, d_imgs, d_tbls, d_segs + nshort, cap, forced,
+                                                           ws + P.off_destuff, d_coef, status_out);
   }
   if (!P.msegs.empty()) {
     // Multi-scan images (coefficients zeroed above): one launch per dependency level.  The scans of one level share
@@ -1428,6 +1890,14 @@ extern "C" int pg_jpeg_parse_multiscan(const uint8_t* data_host, int64_t bytes, 
 
 extern "C" int pg_jpeg_scans(const uint8_t* data_host, int64_t bytes, pg_jpeg_scan* out, int32_t cap) {
   return pg::jpeg_scans(data_host, bytes, out, cap);
+}
+
+extern "C" int pg_jpeg_set_schedule(int32_t mode, int32_t chunk_bytes) { return pg::jpeg_set_schedule(mode, chunk_bytes); }
+
+extern "C" int64_t pg_jpeg_entropy_host(const uint8_t* packed_host, const int64_t* offsets_host,
+                                        const pg_jpeg_info* infos_host, int32_t n, int32_t chunk_bytes, int16_t* coef_out,
+                                        int32_t* status_out, int32_t* rounds_out) {
+  return pg::jpeg_entropy_host(packed_host, offsets_host, infos_host, n, chunk_bytes, coef_out, status_out, rounds_out);
 }
 
 extern "C" size_t pg_jpeg_workspace_bytes(const pg_jpeg_info* infos_host, int32_t n, int64_t packed_bytes) {

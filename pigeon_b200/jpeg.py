@@ -6,8 +6,9 @@ pretrain_dataset.py:109-161).
     imgs = decode_jpeg([open(p, 'rb').read() for p in paths], 'cuda')     # CUDA uint8 [H, W, 3] views into one arena
 
 The headers are parsed on the host (`parse`); the compressed bytes of the whole batch go to the device in one copy and
-three launches decode them.  Files outside the decoded subset (progressive, 12-bit, CMYK, RGB-transform, other
-sampling layouts) and corrupt files raise `ValueError` naming every such index and its reason.
+three or four launches decode them (a long entropy-coded segment, such as a photo without restart markers, is decoded
+by a whole CTA in self-synchronising chunks).  Files outside the decoded subset (progressive, 12-bit, CMYK,
+RGB-transform, other sampling layouts) and corrupt files raise `ValueError` naming every such index and its reason.
 
 With `multiscan=True`, progressive files and sequential files of several scans are decoded too, to the same bytes as
 Pillow, when every coefficient is sent and fully refined (what encoders write; libjpeg smooths the blocks of the other
@@ -73,6 +74,40 @@ def scans(data: Encoded) -> List[_lib.JpegScan]:
     if n < 0:
         raise ValueError(lib.pg_last_error().decode())
     return list(out[:n])
+
+
+def set_schedule(mode: int, chunk_bytes: int = 0) -> None:
+    """Huffman-decode kernel of single-scan segments, process-wide (pg_jpeg_set_schedule): 0 = automatic, 1 = one thread
+    per segment, 2 = chunked for every segment; `chunk_bytes` > 0 forces the chunk size.  For tests and A/B benchmarks:
+    every schedule gives the same bytes."""
+    check(load().pg_jpeg_set_schedule(int(mode), int(chunk_bytes)), "pg_jpeg_set_schedule")
+
+
+def entropy_host(files: Sequence[Encoded], chunk_bytes: int = 0):
+    """The entropy decode of single-scan files on the CPU (pg_jpeg_entropy_host): chunk_bytes 0 = one pass per segment,
+    > 0 = the chunked decoder at that chunk size, < 0 = at the automatic size.  Returns (int16 coefficient blocks
+    [blocks, 64] of the parsed-OK files in order, status per file, synchronisation rounds per file)."""
+    lib = load()
+    bufs = [bytes(f) for f in files]
+    n = len(bufs)
+    infos = (_lib.JpegInfo * n)(*[parse(b)[0] for b in bufs])
+    packed = np.frombuffer(b"".join(bufs), dtype=np.uint8)
+    offsets = np.concatenate([[0], np.cumsum([len(b) for b in bufs])]).astype(np.int64)
+    status = np.zeros(n, dtype=np.int32)
+    rounds = np.zeros(n, dtype=np.int32)
+    nblocks = 0
+    for i in infos:
+        if i.status == OK:
+            three = i.components == 3
+            hmax, vmax = (i.h_samp[0], i.v_samp[0]) if three else (1, 1)
+            mcus = -(-i.width // (8 * hmax)) * -(-i.height // (8 * vmax))
+            nblocks += mcus * (sum(i.h_samp[c] * i.v_samp[c] for c in range(3)) if three else 1)
+    coef = np.zeros((nblocks, 64), dtype=np.int16)
+    got = lib.pg_jpeg_entropy_host(packed.ctypes.data, offsets.ctypes.data, infos, n, chunk_bytes, coef.ctypes.data,
+                                   status.ctypes.data, rounds.ctypes.data)
+    if got != nblocks:
+        raise PigeonB200Error(f"pg_jpeg_entropy_host: {lib.pg_last_error().decode() if got < 0 else got}")
+    return coef, status, rounds
 
 
 class JpegDecoder:

@@ -2,9 +2,12 @@
 """GPU JPEG decoding throughput on one GPU, with the card name and its power limit read in the same run.
 
 Corpora: 640x640 4:2:0 q90 (Street-View-like) and 1024x768 4:2:0 q85 (YFCC-like), each without restart markers and
-with one restart interval per MCU row, at 64, 256 and 1024 files per call (16 distinct synthetic photos, repeated).
-For each: images/s and MB/s of compressed input for decode alone and for decode + pg_preprocess_clip, the per-stage
-kernel times (CUDA events around each launch), and the host-to-device bytes.  For context: Pillow decoding on every
+with one restart interval per MCU row, at 1 and 4 files per call (latency) and 64, 256 and 1024 (throughput; 16
+distinct synthetic photos, repeated).  For each, under the entropy-kernel schedules of pg_jpeg_set_schedule in
+alternation (1 = one thread per segment, 0 = automatic, 2 = chunked everywhere; `--reps` times): images/s and MB/s of
+compressed input for decode alone and for decode + pg_preprocess_clip, the per-stage kernel times (CUDA events around
+each launch: jpeg_entropy for one thread per segment, jpeg_entropy_chunked for the chunked kernel), and the
+host-to-device bytes.  Per corpus, the chunked decoder's synchronisation rounds (maximum and mean over the files).  For context: Pillow decoding on every
 host core followed by the same GPU pre-processing, and a CLIPEmbedding (ViT-L/14-336) pass from bytes against the same
 pass from pre-decoded host pixels.  Prints one JSON line per measurement.
 
@@ -12,7 +15,7 @@ pass from pre-decoded host pixels.  Prints one JSON line per measurement.
 10-scan script, no restart markers) through the multi-scan path (`jpeg_multiscan=True`), with the kernel time of each
 dependency level, against the host route (Pillow on every host core + the same GPU pre-processing).
 
-    python tools/jpeg_bench.py [--multiscan] [--iters 10] [--warmup 3] [--out DIR]
+    python tools/jpeg_bench.py [--multiscan] [--iters 10] [--warmup 3] [--reps 2] [--out DIR]
 """
 import argparse
 import ctypes as C
@@ -87,11 +90,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--out", default=None, help="also write the JSON lines to DIR/jpeg_bench.jsonl")
     ap.add_argument("--multiscan", action="store_true", help="progressive corpora through the multi-scan path")
+    ap.add_argument("--reps", type=int, default=2, help="alternations of the entropy-kernel schedules per workload")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("jpeg_bench needs a CUDA device")
     from PIL import Image
-    from pigeon_b200.jpeg import JpegDecoder
+    from pigeon_b200.jpeg import JpegDecoder, entropy_host, set_schedule
     from pigeon_b200.preprocess import ClipImageProcessor
     dev = torch.device("cuda:0")
     gpu, power = card()
@@ -112,17 +116,31 @@ def main():
     for cname, (h, w, q) in (corpora.items() if not args.multiscan else ()):
         for restart in (False, True):
             distinct = corpus(h, w, q, restart)
-            for n in (64, 256, 1024):
+            # synchronisation rounds of the chunked decoder at its automatic chunk size, from the host entry that runs
+            # the kernel's chunk functions in its order of rounds (the counts do not depend on the device)
+            _, _, rounds = entropy_host(distinct, -1)
+            emit(dict(corpus=cname, restart_rows=restart, files=len(distinct), sync_rounds_max=int(rounds.max()),
+                      sync_rounds_mean=round(float(rounds.mean()), 2),
+                      note="rounds per file: the most any of its segments took"))
+            for n in (1, 4, 64, 256, 1024):
                 files = [distinct[i % len(distinct)] for i in range(n)]
                 mb = sum(len(f) for f in files) / 1e6
-                t_dec = timed(lambda: dec.decode(files), args.iters, args.warmup)
-                t_pre = timed(lambda: proc(images=files), args.iters, args.warmup)
-                stages = stage_ms(lambda: dec.decode(files))
-                emit(dict(corpus=cname, restart_rows=restart, images=n, compressed_mb=round(mb, 3),
-                          h2d_bytes=sum(len(f) for f in files),
-                          decode_ms=round(t_dec * 1e3, 3), decode_img_s=round(n / t_dec, 1), decode_mb_s=round(mb / t_dec, 1),
-                          decode_pre_ms=round(t_pre * 1e3, 3), decode_pre_img_s=round(n / t_pre, 1),
-                          decode_pre_mb_s=round(mb / t_pre, 1), stage_ms=stages))
+                iters = args.iters * (10 if n <= 4 else 1)
+                # the schedules alternate within the job: 1 = one thread per segment (the previous decoder),
+                # 0 = automatic, 2 = chunked for every segment
+                for rep in range(args.reps):
+                    for sched in (1, 0, 2):
+                        set_schedule(sched, 0)
+                        t_dec = timed(lambda: dec.decode(files), iters, args.warmup)
+                        t_pre = timed(lambda: proc(images=files), iters, args.warmup)
+                        stages = stage_ms(lambda: dec.decode(files))
+                        emit(dict(corpus=cname, restart_rows=restart, images=n, schedule=sched, rep=rep,
+                                  compressed_mb=round(mb, 3), h2d_bytes=sum(len(f) for f in files),
+                                  decode_ms=round(t_dec * 1e3, 3), decode_img_s=round(n / t_dec, 1),
+                                  decode_mb_s=round(mb / t_dec, 1), decode_pre_ms=round(t_pre * 1e3, 3),
+                                  decode_pre_img_s=round(n / t_pre, 1), decode_pre_mb_s=round(mb / t_pre, 1),
+                                  stage_ms=stages))
+                set_schedule(0, 0)
             # Pillow on every host core, then the same GPU pre-processing (one call of 256 files)
             files = [distinct[i % len(distinct)] for i in range(256)]
             pool = ThreadPoolExecutor(cores)
