@@ -289,6 +289,53 @@ int64_t pg_jpeg_entropy_host(const uint8_t* packed_host, const int64_t* offsets_
                              int32_t n, int32_t chunk_bytes, int16_t* coef_out, int32_t* status_out, int32_t* rounds_out);
 
 /* ---------------------------------------------------------------------------------------------------
+ * PNG decoding (csrc/png.cu): the same `PIL.Image.open(f).convert('RGB')` for PNG files.  Byte-identical to Pillow
+ * for the files it decodes: non-interlaced PNGs of every colour type and bit depth, with or without tRNS.  Alpha is
+ * dropped, 16-bit samples keep their high byte (16-bit grey clips to 255, as Pillow's I;16 -> RGB does), 1/2/4-bit grey
+ * scales to 0..255, and a palette index past PLTE (or a palette image without PLTE) is black.  Interlaced files, APNG,
+ * IDAT chunks that are not consecutive, CRC errors before the first IDAT and text above Pillow's limits are refused
+ * with a status and a reason (DESIGN.md §1).
+ * ------------------------------------------------------------------------------------------------- */
+#define PG_PNG_OK 0
+#define PG_PNG_UNSUPPORTED 1        /* a file outside the decoded subset: interlaced, APNG, split IDAT runs, ... */
+#define PG_PNG_BAD_HEADER 2         /* not a PNG, no or bad IHDR, no IDAT, a CRC error before the first IDAT */
+#define PG_PNG_BAD_ZLIB 3           /* the zlib header or Adler-32 is wrong, or bytes follow the stream */
+#define PG_PNG_BAD_DEFLATE 4        /* an invalid block type, code set, code or distance */
+#define PG_PNG_TRUNCATED 5          /* the stream ends early, or yields fewer bytes than the rows need */
+#define PG_PNG_TOO_LONG 6           /* more than 4096 decompressed bytes after the rows */
+#define PG_PNG_BAD_FILTER 7         /* a row filter type above 4 */
+
+typedef struct pg_png_info {
+  int32_t status;                 /* PG_PNG_OK, PG_PNG_UNSUPPORTED or PG_PNG_BAD_HEADER */
+  int32_t width, height, bit_depth, color_type;   /* IHDR */
+  int32_t channels;               /* samples per pixel: 1 (grey, palette), 2 (grey + alpha), 3 (RGB) or 4 (RGBA) */
+  int32_t bpp;                    /* filter distance in bytes: max(1, channels * bit_depth / 8) */
+  int32_t palette_entries;        /* PLTE entries of a palette image, 0 without PLTE */
+  int32_t idat_chunks;            /* chunks in the run of consecutive IDATs */
+  int64_t row_bytes;              /* bytes per row, without the filter byte */
+  int64_t idat_offset;            /* offset in the file of the first IDAT chunk (its length field) */
+  int64_t zlib_bytes;             /* payload bytes of the IDAT run: the zlib stream */
+  uint8_t palette[256][3];        /* PLTE, zero past palette_entries */
+} pg_png_info;
+
+/* Host-only chunk walk of one file.  Returns info_out->status; when it is not PG_PNG_OK, pg_last_error() names the
+ * reason. */
+int pg_png_parse(const uint8_t* data_host, int64_t bytes, pg_png_info* info_out);
+/* Workspace of pg_png_decode for n parsed files packed into packed_bytes bytes.  0 on error. */
+size_t pg_png_workspace_bytes(const pg_png_info* infos_host, int32_t n, int64_t packed_bytes);
+/* Decodes the files whose info status is PG_PNG_OK, with the arguments of pg_jpeg_decode: one host-to-device copy of
+ * the packed files and three launches (inflate, one warp per stream; unfiltering; RGB conversion into the dst_host
+ * descriptors, which feed pg_preprocess_clip unchanged).  status_out: device i32 [n], the parse status of a skipped
+ * file, else PG_PNG_OK or the stream / filter error of that file (whose destination is then left unwritten). */
+int pg_png_decode(const uint8_t* packed_host, const int64_t* offsets_host, const pg_png_info* infos_host, int32_t n,
+                  const pg_image* dst_host, void* workspace, size_t workspace_bytes, int32_t* status_out, void* stream);
+/* Host-only test entry: pg_png_decode's inflate, unfilter and convert functions on the CPU.  rgb_out (NULL: not
+ * returned) receives the height x width x 3 bytes of every image with an OK info, in batch order (a failed image's
+ * bytes are unspecified); status_out[n] as pg_png_decode's.  Returns the bytes of rgb_out, or -1 (pg_last_error()). */
+int64_t pg_png_decode_host(const uint8_t* packed_host, const int64_t* offsets_host, const pg_png_info* infos_host,
+                           int32_t n, uint8_t* rgb_out, int32_t* status_out);
+
+/* ---------------------------------------------------------------------------------------------------
  * Fine-tune step, head-only part ("next" row N1 with a frozen or absent base model): what loss.backward() and
  * torch.optim.AdamW.step() do for cell_layer in reference training/train_eval_loop.py:187,215-221.
  * ------------------------------------------------------------------------------------------------- */

@@ -44,6 +44,7 @@ SOURCES = [
     "optics.cu",
     "geo_metrics.cu",
     "jpeg.cu",
+    "png.cu",
 ]
 
 NVCC_FLAGS = [

@@ -104,6 +104,13 @@ class JpegScan(C.Structure):
                 ("al", c_int32), ("restart_interval", c_int32), ("num_segments", c_int32), ("level", c_int32)]
 
 
+class PngInfo(C.Structure):
+    _fields_ = [("status", c_int32), ("width", c_int32), ("height", c_int32), ("bit_depth", c_int32),
+                ("color_type", c_int32), ("channels", c_int32), ("bpp", c_int32), ("palette_entries", c_int32),
+                ("idat_chunks", c_int32), ("row_bytes", c_int64), ("idat_offset", c_int64), ("zlib_bytes", c_int64),
+                ("palette", (C.c_uint8 * 3) * 256)]
+
+
 class GemmProblem(C.Structure):
     _fields_ = [("M", c_int32), ("N", c_int32), ("K", c_int32), ("a", c_void_p), ("lda", c_int32), ("w", c_void_p),
                 ("ldw", c_int32), ("out", c_void_p), ("ldo", c_int32), ("bias", c_void_p), ("epilogue", c_int32),
@@ -184,6 +191,11 @@ SIGNATURES = {
     "pg_jpeg_set_schedule": (c_int32, [c_int32, c_int32]),
     "pg_jpeg_entropy_host": (c_int64, [c_void_p, c_void_p, C.POINTER(JpegInfo), c_int32, c_int32, c_void_p, c_void_p,
                                        c_void_p]),
+    "pg_png_parse": (c_int32, [c_void_p, c_int64, C.POINTER(PngInfo)]),
+    "pg_png_workspace_bytes": (c_size_t, [C.POINTER(PngInfo), c_int32, c_int64]),
+    "pg_png_decode": (c_int32, [c_void_p, c_void_p, C.POINTER(PngInfo), c_int32, c_void_p, c_void_p, c_size_t, c_void_p,
+                                c_void_p]),
+    "pg_png_decode_host": (c_int64, [c_void_p, c_void_p, C.POINTER(PngInfo), c_int32, c_void_p, c_void_p]),
     "pg_head_loss_grad": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_double,
                                     c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pg_head_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,

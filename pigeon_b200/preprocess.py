@@ -11,7 +11,9 @@ Images may also be encoded files (`bytes` / `bytearray` / `memoryview`).  Baseli
 JPEG parser does not decode) is decoded by Pillow on the host, the reference's own decoder, so the pixels are the same
 either way.  `gpu_decoded` / `host_decoded` count the two routes.  A JPEG with corrupt entropy-coded data raises.
 `jpeg_multiscan=True` sends progressive and multi-scan JPEGs to the GPU decoder as well (opt-in until it is measured at
-least as fast as the host route on progressive photos; DESIGN.md §1).
+least as fast as the host route on progressive photos; DESIGN.md §1).  `png=True` decodes PNGs on the GPU
+(pigeon_b200.png); a PNG outside its subset, or whose stream the device refuses, is decoded by Pillow in the same call,
+so pixels and exceptions are those of the default route either way.
 `square_crop=True` (a keyword of the call) first cuts every decoded image to its centred square, the reference's
 `BenchmarkDataset._crop_images` (benchmark_dataset.py:52-66): a strided view of a device image, a slice of a host one.
 """
@@ -24,6 +26,7 @@ import numpy as np
 import torch
 
 from . import _lib, jpeg
+from . import png as _png
 from ._lib import PigeonB200Error, check, current_stream_ptr, load
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
@@ -56,10 +59,14 @@ def _square(img):
     return img[h0:h0 + s, w0:w0 + s]
 
 
-def route_encoded(data, multiscan: bool = False) -> tuple:
-    """('gpu', info) for a file the GPU JPEG decoder takes, ('host', info) for one Pillow decodes on the host (PNG,
-    progressive JPEG unless `multiscan`, anything else the parser does not decode); ValueError for a JPEG with corrupt
-    entropy data."""
+def route_encoded(data, multiscan: bool = False, png: bool = False) -> tuple:
+    """('gpu', info) for a file the GPU JPEG decoder takes, ('host', info) for one Pillow decodes on the host (PNG unless
+    `png`, progressive JPEG unless `multiscan`, anything else the parser does not decode); ValueError for a JPEG with
+    corrupt entropy data.  With `png`, a file with the PNG signature is ('gpu', its pg_png_info) when `png.parse`
+    accepts it and ('host', info) otherwise."""
+    if png and _png.is_png(data):
+        info, _ = _png.parse(data)
+        return ("gpu" if info.status == _png.OK else "host"), info
     info, reason = jpeg.parse(data, multiscan)
     if info.status == jpeg.OK:
         return "gpu", info
@@ -71,14 +78,16 @@ def route_encoded(data, multiscan: bool = False) -> tuple:
 class ClipImageProcessor:
     """Call-compatible with the way the reference uses `CLIPProcessor` for images: `proc(images=..., return_tensors='pt')`
     returns a dict with 'pixel_values' (here a CUDA tensor).  `dtype=torch.float16` writes the tower's input type directly.
-    `jpeg_multiscan=True` decodes encoded progressive and multi-scan JPEGs on the GPU instead of with Pillow.
+    `jpeg_multiscan=True` decodes encoded progressive and multi-scan JPEGs on the GPU instead of with Pillow, `png=True`
+    encoded PNGs (the ones the device refuses are still decoded by Pillow, and counted in `host_decoded`).
     `proc(images, square_crop=True)` cuts each image to its centred square before the resize (BenchmarkDataset)."""
 
     def __init__(self, size: int = 336, image_mean: Sequence[float] = CLIP_MEAN, image_std: Sequence[float] = CLIP_STD,
                  device: Union[str, torch.device] = "cuda", dtype: torch.dtype = torch.float32,
-                 jpeg_multiscan: bool = False):
+                 jpeg_multiscan: bool = False, png: bool = False):
         self.size = int(size)
         self.jpeg_multiscan = bool(jpeg_multiscan)
+        self.png = bool(png)
         self.mean = np.asarray(image_mean, dtype=np.float64).astype(np.float32)
         self.std = np.asarray(image_std, dtype=np.float64).astype(np.float32)
         self.device = torch.device(device)
@@ -90,6 +99,7 @@ class ClipImageProcessor:
         self._lib = load()
         self._ws = None
         self._jpeg = None
+        self._png = None
         self.gpu_decoded = 0
         self.host_decoded = 0
 
@@ -119,15 +129,21 @@ class ClipImageProcessor:
             images = [images]
         dev = [None] * len(images)
         gpu_idx, gpu_files, gpu_infos = [], [], []
+        png_idx, png_files, png_infos = [], [], []
         for i, img in enumerate(images):
             if isinstance(img, torch.Tensor) and img.is_cuda:
                 dev[i] = _square(img) if square_crop else img
                 continue
             if isinstance(img, (bytes, bytearray, memoryview)):
                 try:
-                    route, info = route_encoded(img, self.jpeg_multiscan)
+                    route, info = route_encoded(img, self.jpeg_multiscan, self.png)
                 except ValueError as e:
                     raise ValueError(f"image {i}: {e}") from None
+                if route == "gpu" and isinstance(info, _lib.PngInfo):
+                    png_idx.append(i)
+                    png_files.append(img)
+                    png_infos.append(info)
+                    continue
                 if route == "gpu":
                     gpu_idx.append(i)
                     gpu_files.append(img)
@@ -146,4 +162,25 @@ class ClipImageProcessor:
             for i, t in zip(gpu_idx, self._jpeg.decode(gpu_files, gpu_infos)):
                 dev[i] = _square(t) if square_crop else t
             self.gpu_decoded += len(gpu_files)
+        if png_files:
+            if self._png is None:
+                self._png = _png.PngDecoder(self.device)
+            try:
+                decoded = self._png.decode(png_files, png_infos)
+            except _png.PngDecodeError as e:
+                decoded = e.images
+            from PIL import Image
+            for i, f, t in zip(png_idx, png_files, decoded):
+                if t is None:                                 # refused by the device: Pillow, as without `png`
+                    img = Image.open(io.BytesIO(bytes(f)))
+                    self.host_decoded += 1
+                    a = _to_u8_rgb(img)
+                    if square_crop:
+                        a = np.ascontiguousarray(_square(a))
+                    t = torch.from_numpy(a).pin_memory().to(self.device, non_blocking=True)
+                else:
+                    self.gpu_decoded += 1
+                    if square_crop:
+                        t = _square(t)
+                dev[i] = t
         return {"pixel_values": self.preprocess_device(dev)}

@@ -3,7 +3,7 @@
 
     python run.py evaluate HEAD.model -l DATASET_DIR [-b BASE.model] [--yfcc] [--metrics]
     python run.py evaluate HEAD.model -l BENCHMARK -b BASE.model [--yfcc] [--metrics] [-w WORKERS]   # config.BENCHMARKS
-    python run.py embed CLIP.model -l DATASET_DIR [--jpeg-multiscan]                             # image column + index
+    python run.py embed CLIP.model -l DATASET_DIR [--jpeg-multiscan] [--png]                     # image column + index
     python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading]     # tower + head (run.py:165-169)
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
 
@@ -14,6 +14,9 @@ PRETAIN_ARGS_YFCC with --yfcc; -r passes its `resume_from_checkpoint` to the tra
 `DatasetDict` with `train` and `val` splits whose rows hold pixel_values, input_ids and attention_mask; the caption synthesis
 of the reference's PretrainDataset is not part of this repository.  Datasets are HF `DatasetDict`s on disk, as in the
 reference (run.py:143-162); none are shipped with either repository.
+
+`--png` (embed, evaluate) decodes PNG files on the GPU too; by default Pillow decodes them on the host.  The pixels are
+the same either way.
 
 `--metrics` (evaluate, finetune) evaluates with `metrics.compute_geoguessr_metrics`, as the reference's evaluate.py and
 train_modes.py do: the full GeoGuessr table, with Country_accuracy against config.COUNTRY_PATH.  Without it only
@@ -38,10 +41,10 @@ logger = logging.getLogger('run')
 
 
 def evaluate(model: str, dataset, yfcc: bool, landmarks: bool = False, base_model: str = None, heading: bool = False,
-             refine: bool = True, metrics=None, num_workers: int = 0):
+             refine: bool = True, metrics=None, num_workers: int = 0, png: bool = False):
     """reference evaluation/evaluate.py:10-86.  A BenchmarkDataset or EvalDataset is read as encoded files and
-    pre-processed on the GPU batch by batch; the model's `panorama` is the dataset's (the reference always builds
-    panorama=True, which a benchmark's single view cannot take)."""
+    pre-processed on the GPU batch by batch (`png`: PNG files decoded on the GPU too); the model's `panorama` is the
+    dataset's (the reference always builds panorama=True, which a benchmark's single view cannot take)."""
     from pigeon_b200.benchmark import BenchmarkDataset, EvalDataset
     encoded = isinstance(dataset, (BenchmarkDataset, EvalDataset))
     if encoded and base_model is None:
@@ -84,7 +87,7 @@ def evaluate(model: str, dataset, yfcc: bool, landmarks: bool = False, base_mode
     if encoded:
         from pigeon_b200.preprocess import ClipImageProcessor
         return evaluate_model(full_model, dataset.encoded(), metrics, None, refiner, num_workers=num_workers,
-                              collate_fn=encoded_eval_collate, processor=ClipImageProcessor())
+                              collate_fn=encoded_eval_collate, processor=ClipImageProcessor(png=png))
     return evaluate_model(full_model, dataset, metrics, None, refiner, num_workers=num_workers)
 
 
@@ -103,6 +106,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
     p.add_argument('--jpeg-multiscan', action='store_true',
                    help='embed: decode progressive and multi-scan JPEGs on the GPU too (by default Pillow decodes them)')
+    p.add_argument('--png', action='store_true',
+                   help='embed / evaluate: decode PNG files on the GPU too (by default Pillow decodes them)')
     p.add_argument('-w', '--workers', type=int, default=0,
                    help='evaluate: DataLoader worker processes (they read the image files of a benchmark or raw split)')
     p.add_argument('--metrics', action='store_true',
@@ -126,7 +131,8 @@ def main(argv=None):
     if args.mode == 'evaluate' and not os.path.isdir(load) and os.path.isfile(cfg.BENCHMARKS):   # run.py:158-162
         from pigeon_b200.benchmark import BenchmarkDataset
         print(evaluate(args.name, BenchmarkDataset(load), args.yfcc, args.landmarks, base_model=args.base,
-                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args), num_workers=args.workers))
+                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args), num_workers=args.workers,
+                       png=args.png))
         return
     from datasets import DatasetDict
     dataset = DatasetDict.load_from_disk(load)
@@ -145,9 +151,10 @@ def main(argv=None):
                            metrics=metrics_fn(args))                                                          # run.py:169
     elif args.mode == 'embed':
         kw = {}
-        if args.jpeg_multiscan:
+        if args.jpeg_multiscan or args.png:
             from pigeon_b200.preprocess import ClipImageProcessor
-            kw['processor'] = ClipImageProcessor(device='cuda', dtype=torch.float16, jpeg_multiscan=True)
+            kw['processor'] = ClipImageProcessor(device='cuda', dtype=torch.float16, jpeg_multiscan=args.jpeg_multiscan,
+                                                 png=args.png)
         model = CLIPEmbedding(args.name, load_checkpoint=True, panorama=not args.yfcc, **kw)    # run.py:126-129
         # EmbedDataset semantics (embed_dataset.py:17-22): data['image'] and data['index'] of each split; the files stay
         # encoded until the GPU decodes them
@@ -162,7 +169,8 @@ def main(argv=None):
             from pigeon_b200.benchmark import EvalDataset
             split = EvalDataset(split)
         print(evaluate(args.name, split, args.yfcc, args.landmarks, base_model=args.base,
-                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args), num_workers=args.workers))
+                       heading=args.heading, refine=args.refine, metrics=metrics_fn(args), num_workers=args.workers,
+                       png=args.png))
 
 
 if __name__ == '__main__':

@@ -96,6 +96,7 @@ def main():
     ap.add_argument("--workers", type=int, default=4)
     ap.add_argument("--threads", type=int, default=8)
     ap.add_argument("--repeats", type=int, default=2)
+    ap.add_argument("--png", action="store_true", help="also measure ClipImageProcessor(png=True)")
     ap.add_argument("--out", default=None, help="also write the JSON lines to DIR/benchmark_eval_bench.jsonl")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -142,30 +143,37 @@ def run(args, files, tmp, emit):
     mb = sum(len(f[1]) for f in files) / 1e6
 
     model, refiner = model_and_refiner()
-    proc = ClipImageProcessor()
+    procs = {"default": ClipImageProcessor()}
+    if args.png:
+        procs["png"] = ClipImageProcessor(png=True)
+    proc = procs["default"]
     train_args = SimpleNamespace(per_device_eval_batch_size=args.batch)
 
-    def evaluate():
+    def evaluate(p):
         return loops.evaluate_model(model, ds.encoded(), None, train_args, refiner, num_workers=args.workers,
-                                    collate_fn=loops.encoded_eval_collate, processor=proc)
+                                    collate_fn=loops.encoded_eval_collate, processor=p)
 
-    evaluate()                                                    # warm-up: modules, workspaces, allocator
-    times = []
+    for p in procs.values():
+        evaluate(p)                                               # warm-up: modules, workspaces, allocator
+    times = {r: [] for r in procs}
     for _ in range(args.repeats):
-        torch.cuda.synchronize()
-        t = time.perf_counter()
-        evaluate()
-        torch.cuda.synchronize()
-        times.append(time.perf_counter() - t)
-    t_eval = float(np.median(times))
-    emit(dict(measure="evaluate", images_per_s=round(len(files) / t_eval, 1), seconds=[round(x, 3) for x in times],
-              corpus_mb=round(mb, 1), kinds=kinds, workers=args.workers, refiner=True, metrics="Geocell_accuracy"))
+        for r, p in procs.items():
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            evaluate(p)
+            torch.cuda.synchronize()
+            times[r].append(time.perf_counter() - t)
+    t_evals = {r: float(np.median(ts)) for r, ts in times.items()}
+    for r, ts in times.items():
+        emit(dict(measure="evaluate", route=r, images_per_s=round(len(files) / t_evals[r], 1),
+                  seconds=[round(x, 3) for x in ts], corpus_mb=round(mb, 1), kinds=kinds, workers=args.workers,
+                  refiner=True, metrics="Geocell_accuracy"))
 
     batches = [[f[1] for f in files[i:i + args.batch]] for i in range(0, len(files), args.batch)]
 
-    def gpu_route():
+    def gpu_route(p=proc):
         for b in batches:
-            proc(images=b, square_crop=True)
+            p(images=b, square_crop=True)
         torch.cuda.synchronize()
 
     pool = ThreadPoolExecutor(args.threads)
@@ -179,7 +187,8 @@ def run(args, files, tmp, emit):
             proc(images=list(pool.map(host_decode, b)))
         torch.cuda.synchronize()
 
-    for name, fn in (("decode_gpu", gpu_route), ("decode_host", host_route)):
+    arms = [("decode_gpu", r, (lambda p=p: gpu_route(p))) for r, p in procs.items()] + [("decode_host", None, host_route)]
+    for name, r, fn in arms:
         fn()
         ts = []
         for _ in range(args.repeats):
@@ -188,8 +197,9 @@ def run(args, files, tmp, emit):
             ts.append(time.perf_counter() - t)
         t_dec = float(np.median(ts))
         d = dict(measure=name, images_per_s=round(len(files) / t_dec, 1), seconds=[round(x, 3) for x in ts])
-        if name == "decode_gpu":
-            d["share_of_evaluate"] = round(t_dec / t_eval, 3)
+        if r is not None:
+            d["route"] = r
+            d["share_of_evaluate"] = round(t_dec / t_evals[r], 3)
         emit(d)
     pool.shutdown()
 
