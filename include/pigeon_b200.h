@@ -676,6 +676,26 @@ int pg_dgelu_bf16(const float* dh, const void* u, void* du, int64_t n, void* str
 /* out bf16 [cols, ldo] = transpose(src [rows, lds]); src_type 0 = f32, 1 = f16, 2 = bf16 */
 int pg_transpose_to_bf16(const void* src, int32_t src_type, int64_t lds, void* out, int64_t ldo, int64_t rows, int32_t cols,
                          void* stream);
+/* out f32 [cols] += column sums of x [rows, ldx] (src_type 0 = f32, 2 = bf16): the bias gradients of the backward pass. */
+int pg_column_sum_accumulate(const void* x, int32_t src_type, int64_t ldx, float* out, int64_t rows, int32_t cols,
+                             void* stream);
+/* g f32 [n_views, tokens, hidden] = d_emb f32 [n_views, hidden] * (1 / tokens) for every token (backward of the token mean);
+ * hidden % 4 == 0. */
+int pg_token_mean_backward(const float* d_emb, float* g, int32_t n_views, int32_t tokens, int32_t hidden, void* stream);
+/* dpos f32 [tokens, hidden] += sum over views of d_e f32 [n_views, tokens, hidden]; dcls f32 [hidden] (nullable: the text
+ * tower has no class token) += the token-0 part of that sum. */
+int pg_embed_backward(const float* d_e, float* dpos, float* dcls, int32_t n_views, int32_t tokens, int32_t hidden,
+                      void* stream);
+/* Text final_layer_norm backward on the pooled row b * S + argmax(ids[b]) of each caption: that row of g f32 [n * S, hidden]
+ * = dLN(x)/dx . d_pooled[b] (other rows are not written); dgamma / dbeta f32 [hidden] += their gradients, summed over the
+ * captions in order through part f32 [n, 2 * hidden]. */
+int pg_text_pool_ln_backward(const float* x, const float* d_pooled, const float* gamma, const int64_t* ids, int32_t n,
+                             int32_t S, int32_t hidden, float eps, float* g, float* part, float* dgamma, float* dbeta,
+                             void* stream);
+/* dtok f32 [vocab, hidden] += per id the sum of the rows of dx f32 [rows, hidden] holding it (ascending row order, no
+ * atomics); ids outside [0, vocab) are skipped. */
+int pg_token_embedding_grad(const int64_t* ids, const float* dx, int64_t rows, int32_t hidden, int32_t vocab, float* dtok,
+                            void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Prototype clustering: the per-geocell OPTICS-xi of reference dataset_creation/prototype/prototype.py:121-145

@@ -172,6 +172,12 @@ SIGNATURES = {
                                         c_int32, c_float, c_void_p]),
     "pg_dgelu_bf16": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pg_transpose_to_bf16": (c_int32, [c_void_p, c_int32, c_int64, c_void_p, c_int64, c_int64, c_int32, c_void_p]),
+    "pg_column_sum_accumulate": (c_int32, [c_void_p, c_int32, c_int64, c_void_p, c_int64, c_int32, c_void_p]),
+    "pg_token_mean_backward": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
+    "pg_embed_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
+    "pg_text_pool_ln_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_float,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pg_token_embedding_grad": (c_int32, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p]),
     "pg_head_pack_weight": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p]),
     "pg_head_workspace_bytes": (c_size_t, [c_int32, c_int32]),
     "pg_head_forward": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32,

@@ -566,4 +566,39 @@ int pg_transpose_to_bf16(const void* src, int32_t src_type, int64_t lds, void* o
   return transpose_to_bf16(src, src_type, lds, out, ldo, rows, cols, 0, 0, 0, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pg_column_sum_accumulate(const void* x, int32_t src_type, int64_t ldx, float* out, int64_t rows, int32_t cols,
+                             void* stream) {
+  if (!x || !out) { set_last_error("pg_column_sum_accumulate: null argument"); return 1; }
+  return column_sum_accumulate(x, src_type, ldx, out, rows, cols, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pg_token_mean_backward(const float* d_emb, float* g, int32_t n_views, int32_t tokens, int32_t hidden, void* stream) {
+  if (!d_emb || !g) { set_last_error("pg_token_mean_backward: null argument"); return 1; }
+  return token_mean_backward(d_emb, g, n_views, tokens, hidden, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pg_embed_backward(const float* d_e, float* dpos, float* dcls, int32_t n_views, int32_t tokens, int32_t hidden,
+                      void* stream) {
+  if (!d_e || !dpos) { set_last_error("pg_embed_backward: null argument"); return 1; }
+  return embed_backward(d_e, dpos, dcls, n_views, tokens, hidden, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pg_text_pool_ln_backward(const float* x, const float* d_pooled, const float* gamma, const int64_t* ids, int32_t n,
+                             int32_t S, int32_t hidden, float eps, float* g, float* part, float* dgamma, float* dbeta,
+                             void* stream) {
+  if (!x || !d_pooled || !gamma || !ids || !g || !part || !dgamma || !dbeta) {
+    set_last_error("pg_text_pool_ln_backward: null argument");
+    return 1;
+  }
+  return text_pool_ln_backward(x, d_pooled, gamma, reinterpret_cast<const long long*>(ids), n, S, hidden, eps, g, part, dgamma,
+                               dbeta, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pg_token_embedding_grad(const int64_t* ids, const float* dx, int64_t rows, int32_t hidden, int32_t vocab, float* dtok,
+                            void* stream) {
+  if (!ids || !dx || !dtok) { set_last_error("pg_token_embedding_grad: null argument"); return 1; }
+  return token_embedding_grad(reinterpret_cast<const long long*>(ids), dx, rows, hidden, vocab, dtok,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -73,31 +73,26 @@ def test_transpose_and_dgelu(cuda):
     assert _rel(du.float(), x.grad) < 4e-3                                                 # bf16 rounding of the output
 
 
-@pytest.mark.parametrize("rows,hidden", [(37, 1024), (1000, 256), (5, 768)])
-def test_layernorm_backward(cuda, rows, hidden):
+@pytest.mark.parametrize("code", [0, 1, 2])
+def test_transpose_ragged_shapes_odd_strides_unaligned_source(cuda, code):
+    """Rows and columns of 1, 63, 65, 577 x 4097 (partial 64 x 64 tiles), odd lds / ldo (no paired loads or stores) and a
+    source one element off its pair alignment (the unpaired load path): bf16(src^T) bit for bit, nothing written outside."""
     lib, check, ptr, sp = _lib()
-    g = torch.Generator().manual_seed(rows)
-    x = (torch.randn(rows, hidden, generator=g) * 2 + 0.3).to(cuda)
-    gamma = (1 + 0.2 * torch.randn(hidden, generator=g)).to(cuda)
-    beta = (0.1 * torch.randn(hidden, generator=g)).to(cuda)
-    dy = (torch.randn(rows, hidden, generator=g) * 1e-3).to(cuda)
-    dx0 = (torch.randn(rows, hidden, generator=g) * 1e-3).to(cuda)
-    xr = x.double().requires_grad_(True)
-    gr, br = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
-    torch.nn.functional.layer_norm(xr, (hidden,), gr, br, 1e-5).backward(dy.double())
-    dx = dx0.clone()
-    dg = torch.full((hidden,), 0.5, device=cuda)
-    db = torch.full((hidden,), -0.25, device=cuda)
-    dx16 = torch.empty(rows, hidden, device=cuda, dtype=torch.bfloat16)
-    check(lib.pg_layernorm_backward(ptr(dy), ptr(x), ptr(gamma), ptr(dx), 1, ptr(dg), ptr(db), ptr(dx16), rows, hidden, 1e-5,
-                                    sp()), "pg_layernorm_backward")
-    assert _rel(dx, dx0.double() + xr.grad) < 1e-5
-    assert torch.equal(dx16, dx.to(torch.bfloat16))
-    assert _rel(dg - 0.5, gr.grad) < 1e-4 and _rel(db + 0.25, br.grad) < 1e-4
-    dx2 = torch.full_like(dx, float("nan"))
-    check(lib.pg_layernorm_backward(ptr(dy), ptr(x), ptr(gamma), ptr(dx2), 0, None, None, None, rows, hidden, 1e-5, sp()),
-          "pg_layernorm_backward")
-    assert _rel(dx2, xr.grad) < 1e-5
+    dt = (torch.float32, torch.float16, torch.bfloat16)[code]
+    g = torch.Generator().manual_seed(code)
+    for rows in (1, 63, 65, 577):
+        for cols in (1, 63, 65, 4097):
+            for odd in (True, False):
+                lds = cols + (1 - cols % 2 if odd else cols % 2)      # odd, or even with the source offset by one element
+                ldo = rows + (1 - rows % 2 if odd else rows % 2)
+                base = torch.randn(rows * lds + 1, generator=g).to(cuda, dt)
+                src = base[0 if odd else 1:][:rows * lds].view(rows, lds)
+                out = torch.full((cols + 1, ldo), float("nan"), device=cuda, dtype=torch.bfloat16)
+                check(lib.pg_transpose_to_bf16(src.data_ptr(), code, lds, ptr(out), ldo, rows, cols, sp()),
+                      "pg_transpose_to_bf16")
+                ref = src[:, :cols].float().t().to(torch.bfloat16)
+                assert torch.equal(out[:cols, :rows].view(torch.int16), ref.view(torch.int16)), (rows, cols, odd)
+                assert torch.isnan(out[:cols, rows:].float()).all() and torch.isnan(out[cols:].float()).all()
 
 
 @pytest.mark.parametrize("n_views,seq,heads", [(2, 17, 4), (3, 257, 2), (2, 577, 16), (1, 128, 2), (1, 64, 2)])

@@ -24,7 +24,7 @@ def _rel(a, b):
     return ((a - b).norm() / b.norm()).item()
 
 
-def _run(cuda, dims, n_views, seed, std=0.02, fold=True, mutate=None):
+def _run(cuda, dims, n_views, seed, std=0.02, fold=True, mutate=None, pass_size=3):
     from oracle import vit as ovit
     from pigeon_b200 import synthetic
     from pigeon_b200.vit_engine import VitEngine
@@ -35,7 +35,7 @@ def _run(cuda, dims, n_views, seed, std=0.02, fold=True, mutate=None):
     px = torch.randn(n_views, 3, dims.image_size, dims.image_size, generator=g)
     ref_h, ref_layers = ovit.vit_last_hidden_state(sd, px, patch=dims.patch_size, heads=dims.heads, layers=dims.layers,
                                                    eps=dims.ln_eps, return_layers=True)
-    eng = VitEngine(sd, dims, device=cuda, max_views_per_pass=3, fold_layernorm=fold)
+    eng = VitEngine(sd, dims, device=cuda, max_views_per_pass=pass_size, fold_layernorm=fold)
     emb, hid = eng.forward(px.to(cuda), return_hidden=True)
     torch.cuda.synchronize()
     return emb, hid, ref_h
@@ -47,6 +47,19 @@ def test_vit_tiny(cuda, fold):
     from pigeon_b200.vit_engine import VitDims
     dims = VitDims(image_size=56, patch_size=14, hidden=256, heads=4, intermediate=512, layers=2)
     emb, hid, ref_h = _run(cuda, dims, n_views=5, seed=1, std=0.05, fold=fold)
+    assert torch.isfinite(hid).all()
+    assert _rel(hid, ref_h) < REL_TOL, _rel(hid, ref_h)
+    assert _rel(emb, ref_h.mean(1)) < REL_TOL
+
+
+@pytest.mark.parametrize("fold", [True, False])
+def test_vit_336_one_pass_past_the_layernorm_grid_cap(cuda, fold):
+    """30 views of 577 tokens in one pass: 17,310 rows, more than the 16 blocks x 8 warps per SM of the LayerNorm kernels on
+    132 SMs, so their warps loop over several rows; with fold=True this covers the LayerNorm-fold statistics that embed_preln
+    writes for the first GEMM."""
+    from pigeon_b200.vit_engine import VitDims
+    dims = VitDims(image_size=336, patch_size=14, hidden=256, heads=4, intermediate=1024, layers=1)
+    emb, hid, ref_h = _run(cuda, dims, n_views=30, seed=4, std=0.05, fold=fold, pass_size=30)
     assert torch.isfinite(hid).all()
     assert _rel(hid, ref_h) < REL_TOL, _rel(hid, ref_h)
     assert _rel(emb, ref_h.mean(1)) < REL_TOL
