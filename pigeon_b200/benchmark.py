@@ -11,7 +11,8 @@ path is for parity.  `evaluate_model` takes the batched route instead:
 
 The collate reads each row's files on the DataLoader workers; the main process turns a whole batch into pixel_values
 with one processor call (one JPEG decode and one pre-processing launch sequence; files the JPEG parser does not take
-are decoded by Pillow on the host).
+are decoded by Pillow on the host).  `training.train_model` takes the same pair for fine-tuning on raw splits, whose
+rows then also carry the auxiliary label columns their split has (`loops.LABEL_COLUMNS`).
 
 The reference detours through float32 (`np.asarray(image, dtype=np.float32) / 255` before CLIPProcessor, whose
 `to_pil_image` multiplies by 255 and truncates to uint8 again): that round trip is the identity on all 256 values, so
@@ -28,7 +29,7 @@ import pandas as pd
 import torch
 
 from . import config
-from .loops import read_encoded
+from .loops import LABEL_COLUMNS, read_encoded
 
 _processor = None
 
@@ -156,9 +157,11 @@ class EvalDataset(datasets.Dataset):
         return len(self.views) == 4
 
     def encoded_row(self, index: int) -> Dict[str, Any]:
+        """The row's encoded views and every one of `loops.LABEL_COLUMNS` the split has."""
         sample = self._encoded[index]
-        return {'images': [sample[c] for c in self.views], 'square_crop': False,
-                'labels': sample['labels'], 'labels_clf': sample['labels_clf']}
+        row = {'images': [sample[c] for c in self.views], 'square_crop': False}
+        row.update((k, sample[k]) for k in LABEL_COLUMNS if k in sample)
+        return row
 
     def encoded(self) -> EncodedRows:
         return EncodedRows(self)

@@ -117,23 +117,59 @@ def encoded_image_collate(batch):
     return [read_encoded(row['image']) for row in batch], torch.as_tensor([row['index'] for row in batch])
 
 
+# Columns of a row that `SuperGuessr.forward` takes besides the pixels: `labels` and `labels_clf` are in every row, the
+# others only in the splits that carry them (multi-task and heading fine-tuning).
+LABEL_COLUMNS = ('labels', 'labels_clf', 'labels_multi_task', 'labels_climate', 'labels_month', 'heading')
+
+
 def encoded_eval_collate(batch):
-    """collate_fn for `EncodedRows` (pigeon_b200.benchmark: rows of a BenchmarkDataset or EvalDataset): reads every
-    view's file of every row, row by row, and stacks the labels.  No CUDA work, so it may run on DataLoader workers;
-    `encoded_pixel_values` turns the batch into pixel_values in the main process."""
-    return {'files': [read_encoded(im) for row in batch for im in row['images']],
-            'views': len(batch[0]['images']), 'square_crop': bool(batch[0]['square_crop']),
-            'labels': torch.as_tensor(np.stack([np.asarray(row['labels']) for row in batch])),
-            'labels_clf': torch.as_tensor(np.asarray([row['labels_clf'] for row in batch]))}
+    """collate_fn for `EncodedRows` (pigeon_b200.benchmark: rows of a BenchmarkDataset or EvalDataset), in evaluation
+    and in fine-tuning: reads every view's file of every row, row by row, and stacks each of `LABEL_COLUMNS` the rows
+    carry, with the dtype the rows give it.  No CUDA work, so it may run on DataLoader workers; `encoded_pixel_values`
+    turns the batch into pixel_values in the main process."""
+    out = {'files': [read_encoded(im) for row in batch for im in row['images']],
+           'views': len(batch[0]['images']), 'square_crop': bool(batch[0]['square_crop'])}
+    for k in LABEL_COLUMNS:
+        if k in batch[0]:
+            out[k] = torch.as_tensor(np.stack([np.asarray(row[k]) for row in batch]))
+    return out
 
 
 def encoded_pixel_values(batch, processor):
     """A batch of `encoded_eval_collate` -> the model's keyword arguments: pixel_values [B, 3 * views, 336, 336] on
-    the device from one processor call (JPEG decode + pre-processing for the whole batch), labels, labels_clf."""
+    the device from one processor call (JPEG decode + pre-processing for the whole batch) and the batch's label
+    columns."""
     px = processor(images=batch['files'], square_crop=batch['square_crop'])['pixel_values']
     b = len(batch['files']) // batch['views']
-    return {'pixel_values': px.view(b, 3 * batch['views'], px.shape[2], px.shape[3]),
-            'labels': batch['labels'], 'labels_clf': batch['labels_clf']}
+    out = {'pixel_values': px.view(b, 3 * batch['views'], px.shape[2], px.shape[3])}
+    out.update((k, batch[k]) for k in LABEL_COLUMNS if k in batch)
+    return out
+
+
+def encoded_batches(loader: DataLoader, processor):
+    """The batches of `loader` (collate_fn=encoded_eval_collate) as the model's keyword arguments on the device, each
+    decoded and pre-processed on a side stream while the current stream still runs the work queued before it was
+    requested: a training loop that asks for batch i+1 after queueing step i gets the decode of i+1 under step i.
+
+    The current stream waits on the side stream before a batch is handed out, and its tensors are recorded as used
+    there, so their memory is not reused while the step reads them.  Labels go to the device on the side stream too,
+    so the step's own `.to(device)` calls find them there and do not synchronise the host.  The processor's buffers
+    are only touched on the side stream from the first batch on; that batch's work waits for everything queued
+    before it (an evaluation that used the same processor, say)."""
+    dev = processor.device
+    main = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(main)
+    for batch in loader:
+        with torch.cuda.stream(side):
+            out = encoded_pixel_values(batch, processor)
+            for k, v in out.items():
+                if not v.is_cuda:
+                    out[k] = v.pin_memory().to(dev, non_blocking=True)
+        main.wait_stream(side)
+        for v in out.values():
+            v.record_stream(main)
+        yield out
 
 
 def embed_images(loaded_model: Any, dataset, num_workers: int = 0, save_dir: Optional[str] = 'data/landmark_embeddings',

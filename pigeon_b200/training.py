@@ -17,7 +17,7 @@ from torch.utils.data import DataLoader
 from . import _versions
 from . import dist as pdist
 from ._lib import PigeonB200Error, check, current_stream_ptr, load, ptr
-from .loops import evaluate_model
+from .loops import encoded_batches, evaluate_model
 
 logger = logging.getLogger('train')
 
@@ -203,10 +203,18 @@ def _to_batch(data: Any) -> dict:
 
 def train_model(loaded_model: Any, dataset, on_embeddings: bool, yfcc: bool, train_args, metrics: Optional[Callable],
                 patience: Optional[int] = None, should_profile: bool = False, save_path: Optional[str] = None,
-                num_workers: int = 0):
+                num_workers: int = 0, collate_fn=None, processor=None):
     """reference training/train_eval_loop.py:164-253.  `train_args` needs `.learning_rate`,
     `.per_device_train_batch_size`, `.num_train_epochs`, optionally `.gradient_accumulation_steps`,
-    `.per_device_eval_batch_size`.  Returns the trained model (the best one is saved to `save_path` if given)."""
+    `.per_device_eval_batch_size`.  Returns the trained model (the best one is saved to `save_path` if given).
+
+    With `collate_fn=loops.encoded_eval_collate` and a `processor` (preprocess.ClipImageProcessor), the splits yield
+    encoded files (`EvalDataset.encoded()`): each training batch is decoded and pre-processed on the GPU while the
+    previous step runs (`loops.encoded_batches`), and `val` is evaluated the same way.  Sampling, accumulation,
+    evaluation, early stopping and checkpoints are those of the pixel_values route, and so is the sequence of batches
+    for a given torch seed: this route draws no random numbers of its own."""
+    if (collate_fn is None) != (processor is None):
+        raise ValueError('collate_fn and processor go together: the collate yields encoded files, the processor decodes them')
     if train_args is None:
         from .config import TRAIN_ARGS as train_args
     model = loaded_model
@@ -216,7 +224,7 @@ def train_model(loaded_model: Any, dataset, on_embeddings: bool, yfcc: bool, tra
     if pdist.is_distributed():
         sampler = torch.utils.data.distributed.DistributedSampler(train_ds, shuffle=True)
     train_data = DataLoader(train_ds, train_args.per_device_train_batch_size, shuffle=sampler is None, sampler=sampler,
-                            pin_memory=True, num_workers=num_workers)                        # :188-189
+                            pin_memory=collate_fn is None, num_workers=num_workers, collate_fn=collate_fn)   # :188-189
     prior_eval_loss, current_patience = None, 0
     grad_acc_steps = getattr(train_args, 'gradient_accumulation_steps', None) or 1          # :200-201
     logger.warning('Starting training ...')
@@ -227,7 +235,8 @@ def train_model(loaded_model: Any, dataset, on_embeddings: bool, yfcc: bool, tra
         if sampler is not None:
             sampler.set_epoch(epoch)
         combined_loss = None
-        for i, data in enumerate(train_data):                                                # :214
+        batches = train_data if processor is None else encoded_batches(train_data, processor)
+        for i, data in enumerate(batches):                                                   # :214
             output = model(**_to_batch(data))
             model.backward(output.loss)                                                      # :216
             l = output.loss.detach().double()
@@ -238,7 +247,8 @@ def train_model(loaded_model: Any, dataset, on_embeddings: bool, yfcc: bool, tra
         history.append(float(combined_loss) if combined_loss is not None else float('nan'))
         eval_loss = None
         if 'val' in dataset and dataset['val'] is not None:
-            eval_loss = evaluate_model(model, dataset['val'], metrics, train_args, None, yfcc, None, epoch)   # :232
+            eval_loss = evaluate_model(model, dataset['val'], metrics, train_args, None, yfcc, None, epoch,   # :232
+                                       collate_fn=collate_fn, processor=processor)
             if not isinstance(eval_loss, (int, float)):
                 eval_loss = -float((eval_loss['preds_geocell'] == _labels_clf(dataset['val'])).mean())
         if eval_loss is None or prior_eval_loss is None or eval_loss < prior_eval_loss:     # :235-241
@@ -265,7 +275,8 @@ def _labels_clf(ds):
 def finetune_model(model: Any, dataset, multi_task: bool, heading: bool, yfcc: bool, early_stopping: Optional[int] = None,
                    train_args=None, metrics: Optional[Callable] = None, **train_kwargs):
     """reference training/train_modes.py:67-107.  `model`: a HuggingFace model name (loaded with CLIPVisionModel, needs the
-    checkpoint on disk) or an already built `SuperGuessr`."""
+    checkpoint on disk) or an already built `SuperGuessr`.  `train_kwargs` go to `train_model` (`num_workers`, and
+    `collate_fn` with `processor` for splits of encoded files)."""
     from .super_guessr import SuperGuessr
     if isinstance(model, str):
         if 'clip-vit' not in model:

@@ -4,7 +4,8 @@
     python run.py evaluate HEAD.model -l DATASET_DIR [-b BASE.model] [--yfcc] [--metrics]
     python run.py evaluate HEAD.model -l BENCHMARK -b BASE.model [--yfcc] [--metrics] [-w WORKERS]   # config.BENCHMARKS
     python run.py embed CLIP.model -l DATASET_DIR [--jpeg-multiscan] [--png]                     # image column + index
-    python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading]     # tower + head (run.py:165-169)
+    python run.py finetune openai/clip-vit-large-patch14-336 -l DATASET_DIR [-m] [--heading] [-w WORKERS]  # (run.py:165-169)
+    python run.py finetune openai/clip-vit-large-patch14-336 -l RAW_DIR [--jpeg-multiscan] [--png] [-w WORKERS]
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
 
     python run.py pretrain openai/clip-vit-large-patch14-336 -l PRETRAIN_DATASET_DIR [--yfcc] [-r]          # (run.py:154-163)
@@ -15,8 +16,13 @@ PRETAIN_ARGS_YFCC with --yfcc; -r passes its `resume_from_checkpoint` to the tra
 of the reference's PretrainDataset is not part of this repository.  Datasets are HF `DatasetDict`s on disk, as in the
 reference (run.py:143-162); none are shipped with either repository.
 
-`--png` (embed, evaluate) decodes PNG files on the GPU too; by default Pillow decodes them on the host.  The pixels are
-the same either way.
+`finetune` trains the tower and head (`training.finetune_model`).  A split whose rows hold encoded `image` columns
+(`image`..`image_4`, with `labels`, `labels_clf` and any auxiliary label columns) and no `pixel_values` is wrapped in
+`benchmark.EvalDataset`, as the reference's `EvalDataset.transform` wraps train, val and test; each batch is then decoded
+and pre-processed on the GPU while the previous step trains.  Splits that hold `pixel_values` are trained on as they are.
+
+`--png` (embed, evaluate, finetune) decodes PNG files on the GPU too, `--jpeg-multiscan` (embed, finetune) progressive
+and multi-scan JPEGs; by default Pillow decodes them on the host.  The pixels are the same either way.
 
 `--metrics` (evaluate, finetune) evaluates with `metrics.compute_geoguessr_metrics`, as the reference's evaluate.py and
 train_modes.py do: the full GeoGuessr table, with Country_accuracy against config.COUNTRY_PATH.  Without it only
@@ -105,11 +111,13 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument('-m', '--multitask', action='store_true')
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
     p.add_argument('--jpeg-multiscan', action='store_true',
-                   help='embed: decode progressive and multi-scan JPEGs on the GPU too (by default Pillow decodes them)')
+                   help='embed / finetune: decode progressive and multi-scan JPEGs on the GPU too (by default Pillow '
+                        'decodes them)')
     p.add_argument('--png', action='store_true',
-                   help='embed / evaluate: decode PNG files on the GPU too (by default Pillow decodes them)')
+                   help='embed / evaluate / finetune: decode PNG files on the GPU too (by default Pillow decodes them)')
     p.add_argument('-w', '--workers', type=int, default=0,
-                   help='evaluate: DataLoader worker processes (they read the image files of a benchmark or raw split)')
+                   help='evaluate / finetune: DataLoader worker processes (they read the image files of a benchmark or '
+                        'raw split)')
     p.add_argument('--metrics', action='store_true',
                    help='evaluate / finetune: report compute_geoguessr_metrics (needs config.COUNTRY_PATH)')
     return p
@@ -121,6 +129,13 @@ def metrics_fn(args):
         return None
     from pigeon_b200.metrics import compute_geoguessr_metrics
     return compute_geoguessr_metrics
+
+
+def is_raw_split(split) -> bool:
+    """A split of encoded images (an `image` column, the reference's raw holdout and fine-tuning splits) rather than of
+    pre-processed `pixel_values`."""
+    columns = getattr(split, 'column_names', None) or ()
+    return 'image' in columns and 'pixel_values' not in columns
 
 
 def main(argv=None):
@@ -147,8 +162,15 @@ def main(argv=None):
             finetune_on_embeddings(ds, multi_task=args.multitask, heading=args.heading, yfcc=args.yfcc,
                                    metrics=metrics_fn(args))                                                 # run.py:175
         else:
+            kw = {}
+            if 'train' in ds and is_raw_split(ds['train']):                  # EvalDataset.transform (eval_dataset.py:77-94)
+                from pigeon_b200.benchmark import EvalDataset
+                from pigeon_b200.preprocess import ClipImageProcessor
+                ds = {k: EvalDataset(v).encoded() for k, v in ds.items()}
+                kw = dict(collate_fn=encoded_eval_collate,
+                          processor=ClipImageProcessor(jpeg_multiscan=args.jpeg_multiscan, png=args.png))
             finetune_model(args.name, ds, multi_task=args.multitask, heading=args.heading, yfcc=args.yfcc,
-                           metrics=metrics_fn(args))                                                          # run.py:169
+                           metrics=metrics_fn(args), num_workers=args.workers, **kw)                         # run.py:169
     elif args.mode == 'embed':
         kw = {}
         if args.jpeg_multiscan or args.png:
@@ -164,8 +186,7 @@ def main(argv=None):
     else:
         split = dataset['test'] if 'test' in dataset else dataset[list(dataset.keys())[-1]]
         split = split.with_format('torch')
-        columns = getattr(split, 'column_names', None) or ()
-        if 'image' in columns and 'pixel_values' not in columns:                               # raw holdout split
+        if is_raw_split(split):
             from pigeon_b200.benchmark import EvalDataset
             split = EvalDataset(split)
         print(evaluate(args.name, split, args.yfcc, args.landmarks, base_model=args.base,
