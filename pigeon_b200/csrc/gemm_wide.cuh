@@ -14,14 +14,18 @@
 //
 // CTA = 384 threads, 1 CTA / SM, grid = min(#SM, #tiles); the CTA's i-th tile is blockIdx.x + i * gridDim.x, row-major
 // (m_blk = tile / n_blocks) as in the other kernels:
-//   warpgroup 0     TMA producer (one lane, 24 registers): global -> 3-stage ring (A 128 x 64, W 256 x 64, 128B swizzle)
+//   warpgroup 0     producer (24 registers): one lane runs the TMA loads global -> 3-stage ring (A 128 x 64, W 256 x 64,
+//                   128B swizzle); for the fp16 output warps 1-3 write each tile's epilogue operands (bias, colsum and
+//                   the LayerNorm sums of its rows) into one of two operand buffers, a tile ahead of the consumers
 //   warpgroups 1, 2 consumers (240 registers each): both read every stage, so a stage's empty barrier counts their 8 warps
 //
 // The price is the epilogue overlap that ping-pong buys: both consumers finish a tile together and the tensor cores idle
 // during its epilogue.  The epilogue is kept short: it runs on the accumulator fragment in registers, and every global
 // access of the tile goes through the TMA unit, issued by one lane of the consumer and asynchronous to the other threads.
 //   fp16 output   bias / LayerNorm, quick-GELU, fp16 round to nearest into the consumer's 128B-swizzled staging tile, one
-//                 TMA store per 64 x 64 box while the producer already fills the ring for the next tile.
+//                 TMA store per 64 x 64 box while the producer already fills the ring for the next tile.  Bias, colsum
+//                 and the LayerNorm sums come from the tile's operand buffer, written during the mainloop: the epilogue
+//                 does not wait on global memory.
 //   fp32 residual the consumer's 64 x 256 part in four 64-column steps.  A step's residual (two 64 x 32 fp32 boxes) comes
 //                 in by TMA into one of two step buffers; out = (acc + bias) + resid is written over it and stored by
 //                 TMA; the fp16 copy (EPI_F32_BIAS_RESID_STATS) goes through one 64 x 64 fp16 box.  The residual of
@@ -36,8 +40,9 @@
 // Shared memory (1024 bytes of alignment slack and 256 of mbarriers on top):
 //   ring          3 x (16 KB A + 32 KB W)                                                               147 456
 //   fp16 output   staging, one per consumer: 64 rows x 256 fp16 columns as four 64 x 64 boxes (8 KB)  2 x 32 768
+//                 operand buffers: bias [256], colsum [256] and (s1, s2) [128] fp32                      2 x  3 072
 //   fp32 residual one per consumer: 2 step buffers of 64 x 64 fp32 (16 KB) + one 64 x 64 fp16 box        2 x 40 960
-// 214 272 and 230 656 bytes of the 232 448 a block may have.
+// 220 416 and 230 656 bytes of the 232 448 a block may have.
 #pragma once
 #include "gemm.h"
 #include "gemm_epilogue.cuh"
@@ -70,8 +75,13 @@ constexpr int kResBoxBytes = kBoxRows * kResBoxCols * 4;
 constexpr int kResStepBytes = 2 * kResBoxBytes;             // one 64-column step of the residual / output
 constexpr int kResBytes = 2 * kResStepBytes + kBoxBytes;    // one consumer's two step buffers and fp16 box
 constexpr int kSteps = BLOCK_N / 64;
+// One tile's epilogue operands (fp16 output): bias [256] at 0, colsum [256] at kOpdColsum, the LayerNorm sums (s1, s2) of
+// its 128 rows at kOpdLn.
+constexpr int kOpdColsum = BLOCK_N * 4, kOpdLn = 2 * BLOCK_N * 4;
+constexpr int kOpdBytes = kOpdLn + BLOCK_M * 8;
+constexpr int kOpdThreads = 96;   // warps 1-3 of the producer warpgroup write them
 template <int EPI>
-constexpr int epi_bytes() { return 2 * (EpiTraits<EPI>::kResid ? kResBytes : kOutBytes); }
+constexpr int epi_bytes() { return 2 * (EpiTraits<EPI>::kResid ? kResBytes : kOutBytes + kOpdBytes); }
 template <int EPI>
 constexpr int smem_bytes() { return kStages * kStageBytes + epi_bytes<EPI>() + 1024 /*align slack*/ + 256 /*barriers*/; }
 static_assert(smem_bytes<EPI_F32_BIAS_RESID_STATS>() <= 232448 && smem_bytes<EPI_F16_BIAS>() <= 232448,
@@ -80,26 +90,41 @@ static_assert(kBoxBytes % 1024 == 0 && kStageBytes % 1024 == 0 && kResBoxBytes %
               "128B-swizzled tiles start on 1024-byte boundaries");
 constexpr int kConsumerBar = 1;   // + c: the 128 threads of consumer c
 
-// Bias / colsum pair.  A coherent load (not ld.global.nc, which ptxas may move above a barrier): the epilogue's named
-// barriers then keep each box's loads with that box, instead of all 64 being in flight at once next to the 128 accumulators.
+// Bias pair of the residual epilogue.  A coherent load (not ld.global.nc, which ptxas may move above a barrier): the
+// epilogue's named barriers then keep each step's loads with that step, next to the 128 accumulators.
 __device__ __forceinline__ float2 ldg_f2(const float* p) {
   float2 v;
   asm volatile("ld.global.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
   return v;
 }
 
+__device__ __forceinline__ float2 lds_f2(uint32_t saddr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr));
+  return v;
+}
+__device__ __forceinline__ void sts_f2(uint32_t saddr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(x), "f"(y) : "memory");
+}
+
 // LayerNorm consumer: out = ln_a * acc + ln_b * colsum + bias, with (ln_a, ln_b) of the A row (= output row) from the
-// producer's per-128-column partials, summed as epilogue_tile (gemm_epilogue.cuh) sums them.
-__device__ __forceinline__ void ln_coeffs(const GemmArgs& args, int row, float& ln_a, float& ln_b) {
+// producer's per-128-column partials, summed as epilogue_tile (gemm_epilogue.cuh) sums them: ln_sums adds up the row's
+// partials in order, ln_coeffs turns the two sums into the coefficients.
+__device__ __forceinline__ float2 ln_sums(const GemmArgs& args, int row) {
   float s1 = 0.f, s2 = 0.f;
   if (row < args.M) {
     const float2* st = reinterpret_cast<const float2*>(args.stats) + (long)row * args.stats_slots;
-    for (int k = 0; k < args.stats_slots; ++k) {
-      const float2 p = st[k];
+    const float2* end = st + args.stats_slots;
+#pragma unroll 2
+    for (; st < end; ++st) {
+      const float2 p = *st;
       s1 += p.x;
       s2 += p.y;
     }
   }
+  return make_float2(s1, s2);
+}
+__device__ __forceinline__ void ln_coeffs(const GemmArgs& args, float s1, float s2, float& ln_a, float& ln_b) {
   const float inv_k = 1.0f / (float)args.K;
   const float mu = s1 * inv_k;
   const float var = fmaxf(s2 * inv_k - mu * mu, 0.f);
@@ -107,18 +132,55 @@ __device__ __forceinline__ void ln_coeffs(const GemmArgs& args, int row, float& 
   ln_b = -ln_a * mu;
 }
 
-// One consumer warpgroup's epilogue of its 64 x 256 part of the tile.  Thread (warp w, lane l) holds rows r = 16 w + l / 4
-// and r + 8 (wgmma.cuh fragment layout; ln_a / ln_b [h] belong to row r + 8 h), columns 8 j + 2 (l % 4) + {0, 1} for
-// j < 32.  Per element it does exactly what epilogue_tile (gemm_epilogue.cuh) does, in the same order.
+// The epilogue operands of one tile (fp16 output) -> its operand buffer at shared address `opd`, by warps 1-3 of the
+// producer warpgroup while the consumers still run an earlier tile: warp 3 the bias and colsum of the tile's 256 columns
+// (0 past N), warps 1 and 2 the LayerNorm sums (ln_sums) of its rows [0, 64) and [64, 128), one row at a time per lane
+// within the producer's 24 registers; the consumers turn them into (ln_a, ln_b) with ln_coeffs.
 template <int EPI>
-__device__ __forceinline__ void wide_epilogue(const GemmArgs& args, const float (&acc)[BLOCK_N / 2], const float (&ln_a)[2],
-                                              const float (&ln_b)[2], const uint8_t* out_tile, const CUtensorMap* tmap_out,
-                                              int c, int warp_in_group, int lane, int tile_row0, int tile_col0) {
+__device__ __forceinline__ void fill_operands(const GemmArgs& args, uint32_t opd, int warp_in_group, int lane, int tile_row0,
+                                              int tile_col0) {
+  constexpr bool kLn = EpiTraits<EPI>::kLn;
+  if (warp_in_group == 3) {
+#pragma unroll 2
+    for (int i = 0; i < BLOCK_N / 32; ++i) {
+      const int j = 32 * i + lane, col = tile_col0 + j;
+      float b = 0.f, cs = 0.f;
+      if (col < args.N) {
+        if (args.bias != nullptr) b = __ldg(args.bias + col);
+        if (kLn) cs = __ldg(args.colsum + col);
+      }
+      sts_f1(opd + 4 * j, b);
+      if (kLn) sts_f1(opd + kOpdColsum + 4 * j, cs);
+    }
+  } else if (kLn) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = 64 * (warp_in_group - 1) + 32 * h + lane;
+      const float2 s12 = ln_sums(args, tile_row0 + r);
+      sts_f2(opd + kOpdLn + 8 * r, s12.x, s12.y);
+    }
+  }
+}
+
+// One consumer warpgroup's epilogue of its 64 x 256 part of the tile.  Thread (warp w, lane l) holds rows r = 16 w + l / 4
+// and r + 8 (wgmma.cuh fragment layout), columns 8 j + 2 (l % 4) + {0, 1} for j < 32.  Per element it does exactly what
+// epilogue_tile (gemm_epilogue.cuh) does, in the same order.  `opd`: the tile's operand buffer (fill_operands).
+template <int EPI>
+__device__ __forceinline__ void wide_epilogue(const GemmArgs& args, const float (&acc)[BLOCK_N / 2], uint32_t opd,
+                                              const uint8_t* out_tile, const CUtensorMap* tmap_out, int c, int warp_in_group,
+                                              int lane, int tile_row0, int tile_col0) {
   constexpr bool kLn = EpiTraits<EPI>::kLn;
   constexpr bool kGelu = (EPI == EPI_F16_BIAS_QGELU || EPI == EPI_F16_LN_BIAS_QGELU);
   const int rbase = 16 * warp_in_group + (lane >> 2);   // this lane's first row within the consumer's 64
-  const bool tile_in_n = tile_col0 + BLOCK_N <= args.N;
   const bool store_lane = (warp_in_group | lane) == 0;
+  float ln_a[2] = {1.f, 1.f}, ln_b[2] = {0.f, 0.f};    // of rows rbase + 8 h
+  if (kLn) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float2 s12 = lds_f2(opd + kOpdLn + 8 * (64 * c + rbase + 8 * h));
+      ln_coeffs(args, s12.x, s12.y, ln_a[h], ln_b[h]);
+    }
+  }
   if (store_lane) bulk_wait_group_read<0>();   // the previous tile's stores have read the staging tile
   named_barrier_sync(kConsumerBar + c, 128);
   // 16-byte piece q of staging row r sits at piece slot q ^ (r & 7) (the TMA unit's 128-byte swizzle); rows r and r + 8
@@ -127,20 +189,13 @@ __device__ __forceinline__ void wide_epilogue(const GemmArgs& args, const float 
   const int sw = rbase & 7;
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
-    const int col = tile_col0 + 8 * j + 2 * (lane & 3);
+    const uint32_t ocol = opd + (uint32_t)(8 * j + 2 * (lane & 3)) * 4;
     float2 b = make_float2(0.f, 0.f), cs = make_float2(0.f, 0.f);
-    if (kLn) {   // N % 64 == 0 (checked at launch): a column pair is wholly inside or past N
-      if (col < args.N) {
-        cs = ldg_f2(args.colsum + col);
-        b = ldg_f2(args.bias + col);
-      }
+    if (kLn) {
+      cs = lds_f2(ocol + kOpdColsum);
+      b = lds_f2(ocol);
     } else if (args.bias != nullptr) {
-      if (tile_in_n) {
-        b = ldg_f2(args.bias + col);
-      } else {
-        if (col < args.N) b.x = __ldg(args.bias + col);
-        if (col + 1 < args.N) b.y = __ldg(args.bias + col + 1);
-      }
+      b = lds_f2(ocol);
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -158,8 +213,6 @@ __device__ __forceinline__ void wide_epilogue(const GemmArgs& args, const float 
       }
       sts_u1(srow + (uint32_t)(j >> 3) * kBoxBytes + (uint32_t)(8 * h) * 128 + (uint32_t)(((j & 7) ^ sw) << 4), pack_half2(v0, v1));
     }
-    // one box at a time: without the barrier ptxas starts every box's loads and MUFU work at once and spills
-    if ((j & 7) == 7 && j + 1 < BLOCK_N / 8) named_barrier_sync(kConsumerBar + c, 128);
   }
   fence_proxy_async_smem();   // the generic-proxy writes above, before the TMA unit reads them
   named_barrier_sync(kConsumerBar + c, 128);
@@ -170,15 +223,6 @@ __device__ __forceinline__ void wide_epilogue(const GemmArgs& args, const float 
         tma_store_2d(tmap_out, out_tile + q * kBoxBytes, tile_col0 + q * kBoxCols, tile_row0 + 64 * c);
     bulk_commit_group();
   }
-}
-
-__device__ __forceinline__ float2 lds_f2(uint32_t saddr) {
-  float2 v;
-  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr));
-  return v;
-}
-__device__ __forceinline__ void sts_f2(uint32_t saddr, float x, float y) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(x), "f"(y) : "memory");
 }
 
 // Residual of one 64-column step (global columns [col, col + 64) of the consumer's 64 rows from row0) -> a step buffer, as
@@ -316,10 +360,13 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * kABytes;
   uint8_t* smem_out = smem + kStages * kStageBytes;   // the consumers' staging tiles / residual buffers
+  uint8_t* smem_opd = smem_out + 2 * kOutBytes;       // fp16 output: the two operand buffers
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_out + epi_bytes<EPI>());
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
   uint64_t* res_bar = bars + 2 * kStages;   // + 2 c + b: consumer c's step buffer b is loaded
+  uint64_t* opd_full = bars + 2 * kStages;  // + b: operand buffer b is written (fp16 output)
+  uint64_t* opd_empty = opd_full + 2;       // + b: both consumers have read it
 
   const int wg = threadIdx.x >> 7;
   const int warp_in_group = (threadIdx.x >> 5) & 3;
@@ -339,6 +386,11 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     }
     if (kResid)
       for (int i = 0; i < 4; ++i) mbar_init(&res_bar[i], 1);   // the store lane's arrive.expect_tx
+    else
+      for (int b = 0; b < 2; ++b) {
+        mbar_init(&opd_full[b], kOpdThreads);
+        mbar_init(&opd_empty[b], 2);   // the store lane of each consumer
+      }
     fence_mbar_init();
   }
   __syncthreads();
@@ -363,6 +415,18 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
+    } else if (!kResid && warp_in_group > 0) {
+      // the epilogue operands, double-buffered: tile i's are written while the consumers run tile i - 1
+      // (shared-window addresses: generic pointers would take two of the 24 registers each)
+      const uint32_t opd_s = smem_u32(smem_opd), full_s = smem_u32(opd_full), empty_s = smem_u32(opd_empty);
+      for (uint32_t it = 0;; ++it) {
+        const int tile = blockIdx.x + it * gridDim.x;
+        if (tile >= num_tiles) break;
+        const uint32_t b = it & 1;
+        mbar_wait(empty_s + 8 * b, ((it >> 1) & 1) ^ 1);
+        fill_operands<EPI>(args, opd_s + b * kOpdBytes, warp_in_group, lane, tile / n_blocks * BLOCK_M, tile % n_blocks * BLOCK_N);
+        mbar_arrive(full_s + 8 * b);
+      }
     }
     return;
   }
@@ -380,16 +444,10 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint32_t res_phase = 0;
   int stage = 0;
   uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  uint32_t it = 0;   // the CTA's tile count
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
     const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
     const int row0 = m_blk * BLOCK_M + 64 * c;   // the consumer's first row
-    // LayerNorm coefficients of this lane's two rows, before the accumulators are live (with them live the epilogue spills)
-    float ln_a[2] = {1.f, 1.f}, ln_b[2] = {0.f, 0.f};
-    if (EpiTraits<EPI>::kLn) {
-      const int row = row0 + 16 * warp_in_group + (lane >> 2);
-      ln_coeffs(args, row, ln_a[0], ln_b[0]);
-      ln_coeffs(args, row + 8, ln_a[1], ln_b[1]);
-    }
     // The first MMA of the tile overwrites the accumulators (scale-d 0); defining them here ends their live range at the
     // previous tile's epilogue.
     float acc[BLOCK_N / 2];
@@ -434,7 +492,11 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         wide_resid_epilogue<EPI>(args, acc, out_tile, res_bar + 2 * c, res_phase, &tmap_out, &tmap_resid, &tmap_aux, pol, c,
                                  warp_in_group, lane, row0, n_blk * BLOCK_N);
     } else {
-      wide_epilogue<EPI>(args, acc, ln_a, ln_b, out_tile, &tmap_out, c, warp_in_group, lane, m_blk * BLOCK_M, n_blk * BLOCK_N);
+      const int b = it & 1;
+      mbar_wait(&opd_full[b], (it >> 1) & 1);   // written during the mainloop, or earlier
+      wide_epilogue<EPI>(args, acc, smem_u32(smem_opd + b * kOpdBytes), out_tile, &tmap_out, c, warp_in_group, lane,
+                         m_blk * BLOCK_M, n_blk * BLOCK_N);
+      if (store_lane) mbar_arrive(&opd_empty[b]);   // after the epilogue's last barrier: the warpgroup is done reading
     }
   }
   if (store_lane) bulk_wait_group<0>();   // the last tile's stores are complete before the CTA exits

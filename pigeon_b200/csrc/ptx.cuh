@@ -42,9 +42,11 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+// (the uint32_t overloads take the barrier's shared-window address)
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { mbar_arrive(smem_u32(bar)); }
 
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
@@ -52,7 +54,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
                : "memory");
 }
 
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
       "{\n\t"
@@ -61,26 +63,28 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       "selp.u32 %0, 1, 0, p;\n\t"
       "}\n"
       : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
+      : "r"(bar), "r"(parity)
       : "memory");
   return ok != 0;
 }
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) { return mbar_try_wait(smem_u32(bar), parity); }
 
 // A dead-locked wait traps (see PG_SPIN_LIMIT).  The report (block, thread, barrier address, parity) is compiled in only
 // with -DPG_DEADLOCK_REPORT (PG_NVCC_EXTRA="-DPG_DEADLOCK_REPORT" python -m pigeon_b200._build --force): inlined at every
 // wait it costs ~50 instructions per site.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > PG_SPIN_LIMIT) {
 #ifdef PG_DEADLOCK_REPORT
       printf("pigeon_b200: mbarrier dead-lock block=(%d,%d,%d) thread=%d bar=%u parity=%u\n",
-             blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, smem_u32(bar), parity);
+             blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, bar, parity);
 #endif
       __trap();
     }
   }
 }
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
 
 // ----------------------------------------------------------------------------------------------
 // TMA
