@@ -28,7 +28,8 @@ from torch.nn.parameter import Parameter
 from . import _versions, ops
 from ._lib import PigeonB200Error
 from ._lib import check, current_stream_ptr, load, ptr
-from .clip_text import CLIPTextTower, TextDims, _Holder, check_sequence_length
+from .clip_text import CLIPTextTower, TextDims, check_sequence_length
+from .encoder import linear
 from .super_guessr import CLIPVisionTower
 from .vit_engine import VitDims
 from .vit_train import put_grad
@@ -57,10 +58,8 @@ class CLIPModel(nn.Module):
         self._towers = (CLIPTextTower(text_dims), CLIPVisionTower(vision_dims))
         self.text_model = self._towers[0].text_model
         self.vision_model = self._towers[1].vision_model
-        self.visual_projection = _Holder()
-        self.visual_projection.weight = Parameter(torch.zeros(projection_dim, vision_dims.hidden))
-        self.text_projection = _Holder()
-        self.text_projection.weight = Parameter(torch.zeros(projection_dim, text_dims.hidden))
+        self.visual_projection = linear(projection_dim, vision_dims.hidden, bias=False)
+        self.text_projection = linear(projection_dim, text_dims.hidden, bias=False)
         self.logit_scale = Parameter(torch.tensor(LOGIT_SCALE_INIT))
         self._packed = {}
         self.max_train_views = 64    # activation arena of the vision tower's training step (about 0.52 GB per ViT-L/14-336 view)

@@ -15,7 +15,7 @@ import torch
 from . import _lib
 from ._lib import PigeonB200Error, check, current_stream_ptr, load, ptr
 from .clip_text import admissible_keys
-from .vit_train import (LAYER_GRADS, _aligned_empty, _align, layer_grad_shapes, put_grad, put_layer_grads,
+from .vit_train import (carve_saved, flat_grads, grow_aligned, layer_grad_shapes, layers_bwd, put_grad, put_layer_grads,
                         transpose_layers)
 
 
@@ -42,44 +42,18 @@ class TextTrainer:
                                       f"pretraining does); frozen: {frozen[:3]}{' ...' if len(frozen) > 3 else ''}")
 
     def _build_saved(self, n: int, S: int):
-        d = self.dims
-        rows = n * S
-        H, I = d.hidden, d.intermediate
-        per_layer = [("x0", rows * H * 4), ("xn1", rows * H * 2), ("qkv", rows * 3 * H * 2), ("lse2", n * d.heads * S * 4),
-                     ("ao", rows * H * 2), ("x1", rows * H * 4), ("xn2", rows * H * 2), ("u", rows * I * 2),
-                     ("h", rows * I * 2)]
-        total = _align(rows * H * 4) + d.layers * sum(_align(b) for _, b in per_layer)
-        dev = next(self.tower.parameters()).device
-        if self._arena is None or self._arena.numel() < total:
-            self._arena = None
-            self._arena = _aligned_empty(total, dev)
-        base, off = self._arena.data_ptr(), 0
         saved = _lib.TextSaved()
-        saved.x_final = base
-        off += _align(rows * H * 4)
-        layers = (_lib.VitSavedLayer * d.layers)()
-        for l in range(d.layers):
-            for name, b in per_layer:
-                setattr(layers[l], name, base + off)
-                off += _align(b)
-        saved.layers_host = layers
-        self._saved, self._saved_layers, self._shape = saved, layers, (n, S)
+        carve_saved(self, saved, n, S, [("x_final", n * S * self.dims.hidden * 4)])
+        self._saved, self._shape = saved, (n, S)
 
     def _pending_grads(self) -> Dict[str, torch.Tensor]:
-        if self._pending is not None:
-            return self._pending
-        d = self.dims
-        dev = next(self.tower.parameters()).device
-        shapes = [("token_emb", (d.vocab, d.hidden)), ("pos_emb", (d.max_positions, d.hidden)),
-                  ("final_ln_g", (d.hidden,)), ("final_ln_b", (d.hidden,))]
-        for l in range(d.layers):
-            shapes += layer_grad_shapes(l, d.hidden, d.intermediate)
-        offs, total = [], 0
-        for _, shp in shapes:
-            offs.append(total)
-            total += (int(torch.Size(shp).numel()) + 3) // 4 * 4
-        flat = torch.zeros(total, dtype=torch.float32, device=dev)
-        self._pending = {name: flat[o:o + int(torch.Size(shp).numel())].view(shp) for (name, shp), o in zip(shapes, offs)}
+        if self._pending is None:
+            d = self.dims
+            shapes = [("token_emb", (d.vocab, d.hidden)), ("pos_emb", (d.max_positions, d.hidden)),
+                      ("final_ln_g", (d.hidden,)), ("final_ln_b", (d.hidden,))]
+            for l in range(d.layers):
+                shapes += layer_grad_shapes(l, d.hidden, d.intermediate)
+            _, self._pending = flat_grads(shapes, next(self.tower.parameters()).device)
         return self._pending
 
     @torch.no_grad()
@@ -111,20 +85,11 @@ class TextTrainer:
         eng = self.tower.engine()
         transpose_layers(self.tower.text_model.encoder.layers, self.tower._group_versions(), self._wt, self._wt_version)
         g = self._pending_grads()
-        lb = (_lib.VitLayerBwd * d.layers)()
-        for l in range(d.layers):
-            for k, t in self._wt[l].items():
-                setattr(lb[l], k, t.data_ptr())
-            for k in LAYER_GRADS:
-                setattr(lb[l], "d_" + k, g[f"{l}.{k}"].data_ptr())
-        grads = _lib.TextGrads(ptr(g["token_emb"]), ptr(g["pos_emb"]), ptr(g["final_ln_g"]), ptr(g["final_ln_b"]), lb)
-        need = int(self._lib.pg_text_backward_workspace_bytes(eng._handle, n, S))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = _aligned_empty(need, d_pooled.device)
+        grads = _lib.TextGrads(ptr(g["token_emb"]), ptr(g["pos_emb"]), ptr(g["final_ln_g"]), ptr(g["final_ln_b"]),
+                               layers_bwd(self._wt, g, [True] * d.layers))
+        ws = grow_aligned(self, "_ws", int(self._lib.pg_text_backward_workspace_bytes(eng._handle, n, S)), d_pooled.device)
         check(self._lib.pg_text_backward(eng._handle, C.byref(self._saved), ptr(ids), ptr(mask), ptr(d_pooled), n, S,
-                                         C.byref(grads), ptr(self._ws), self._ws.numel(), current_stream_ptr()),
-              "pg_text_backward")
+                                         C.byref(grads), ptr(ws), ws.numel(), current_stream_ptr()), "pg_text_backward")
 
     @torch.no_grad()
     def finalize(self) -> None:

@@ -20,6 +20,7 @@ from . import _lib, _versions, ops
 from ._lib import PigeonB200Error, check, current_stream_ptr, load, ptr
 from .config import (CLIP_EMBED_DIM, CLIP_PRETRAINED_HEAD, CLIP_PRETRAINED_HEAD_YFCC, GEOCELL_PATH, GEOCELL_PATH_YFCC,
                      LABEL_SMOOTHING_CONSTANT)
+from .encoder import EncoderTower, Holder, encoder_holder, norm
 from .model_utils import ModelOutput, TopK
 from .vit_engine import VitDims, VitEngine
 
@@ -31,30 +32,13 @@ NUM_MONTHS = 12
 MONTHS_LOSS_SCALING = 1
 
 
-class _Holder(nn.Module):
-    """Parameter container (no forward): keeps the HF module tree so state_dict() key names match."""
-
-
-def _linear(out_f: int, in_f: int) -> nn.Module:
-    h = _Holder()
-    h.weight = Parameter(torch.zeros(out_f, in_f))
-    h.bias = Parameter(torch.zeros(out_f))
-    return h
-
-
-def _norm(n: int) -> nn.Module:
-    h = _Holder()
-    h.weight = Parameter(torch.ones(n))
-    h.bias = Parameter(torch.zeros(n))
-    return h
-
-
-class CLIPVisionTower(nn.Module):
+class CLIPVisionTower(EncoderTower, nn.Module):
     """Drop-in for HF `CLIPVisionModel` on the path the reference uses (models/clip_embedder.py:26,63;
     evaluation/evaluate.py:36; models/super_guessr.py:137-160,395-398): same parameter names
     (`vision_model.embeddings...`, `vision_model.pre_layrnorm`, `vision_model.encoder.layers.N....`), `.config`,
     `.base_model`, `.vision_model.encoder.layers`, and `tower(pixel_values=...)` -> `.last_hidden_state`.
     fp32 master parameters live here; the fp16 kernel layouts are (re)packed lazily by `VitEngine`."""
+    ENGINE, PASS_LIMIT = VitEngine, "max_views_per_pass"
 
     def __init__(self, dims: VitDims = VitDims(), name_or_path: str = ""):
         super().__init__()
@@ -63,38 +47,20 @@ class CLIPVisionTower(nn.Module):
                                       num_hidden_layers=dims.layers, num_attention_heads=dims.heads,
                                       image_size=dims.image_size, patch_size=dims.patch_size,
                                       layer_norm_eps=dims.ln_eps, _name_or_path=name_or_path)
-        vm = _Holder()
-        emb = _Holder()
+        vm = Holder()
+        emb = Holder()
         emb.class_embedding = Parameter(torch.zeros(dims.hidden))
-        pe = _Holder()
+        pe = Holder()
         pe.weight = Parameter(torch.zeros(dims.hidden, 3, dims.patch_size, dims.patch_size))
         emb.patch_embedding = pe
-        pos = _Holder()
+        pos = Holder()
         pos.weight = Parameter(torch.zeros(dims.tokens, dims.hidden))
         emb.position_embedding = pos
         vm.embeddings = emb
-        vm.pre_layrnorm = _norm(dims.hidden)  # [sic] HF spelling
-        enc = _Holder()
-        layers = []
-        for _ in range(dims.layers):
-            L = _Holder()
-            sa = _Holder()
-            for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
-                setattr(sa, n, _linear(dims.hidden, dims.hidden))
-            L.self_attn = sa
-            L.layer_norm1 = _norm(dims.hidden)
-            mlp = _Holder()
-            mlp.fc1 = _linear(dims.intermediate, dims.hidden)
-            mlp.fc2 = _linear(dims.hidden, dims.intermediate)
-            L.mlp = mlp
-            L.layer_norm2 = _norm(dims.hidden)
-            layers.append(L)
-        enc.layers = nn.ModuleList(layers)
-        vm.encoder = enc
-        vm.post_layernorm = _norm(dims.hidden)  # present in HF checkpoints; unused by PIGEON (pooler_output)
+        vm.pre_layrnorm = norm(dims.hidden)  # [sic] HF spelling
+        vm.encoder = encoder_holder(dims.hidden, dims.intermediate, dims.layers)
+        vm.post_layernorm = norm(dims.hidden)  # present in HF checkpoints; unused by PIGEON (pooler_output)
         self.vision_model = vm
-        self._engine: Optional[VitEngine] = None
-        self._packed_version = None
         self.max_views_per_pass = 256
         self.fold_layernorm = True   # LayerNorm applied in the GEMM epilogues (False = LayerNorm kernels; A/B switch)
 
@@ -115,41 +81,13 @@ class CLIPVisionTower(nn.Module):
             raise PigeonB200Error(f"cannot map HF weights: missing={missing} unexpected={unexpected}")
         return tower
 
-    def _weights_changed(self):
-        self._packed_version = None
-
-    def _weights_version(self):
-        return tuple((p.data_ptr(), p._version, _versions.get(p)) for p in self.parameters())
-
-    def _group_versions(self):
-        """Version key per repack group: "embeddings" (patch / class / position embeddings, pre-LayerNorm) and one per encoder
-        layer — under the reference's fine-tune policy only the last layer moves between optimizer steps."""
-        def key(module_params):
-            return tuple((p.data_ptr(), p._version, _versions.get(p)) for p in module_params)
+    def _repack_groups(self):
+        """The "embeddings" group: patch / class / position embeddings and pre-LayerNorm."""
         vm = self.vision_model
-        groups = {"embeddings": key(list(vm.embeddings.parameters()) + list(vm.pre_layrnorm.parameters()))}
-        for i, layer in enumerate(vm.encoder.layers):
-            groups[i] = key(layer.parameters())
-        return groups
+        return list(vm.embeddings.parameters()) + list(vm.pre_layrnorm.parameters()), vm.encoder.layers
 
-    def engine(self) -> VitEngine:
-        p0 = next(self.parameters())
-        if not p0.is_cuda:
-            raise PigeonB200Error("CLIPVisionTower is on the CPU: move the model with .to('cuda') — the H100 path "
-                                  "has no CPU implementation")
-        v = self._group_versions()
-        if self._engine is None or self._packed_version != v:
-            sd = {k: t.detach() for k, t in self.state_dict().items()}
-            if (self._engine is None or self._engine.device != p0.device
-                    or self._engine.fold_layernorm != bool(self.fold_layernorm)):
-                self._engine = VitEngine(sd, self.dims, device=p0.device, max_views_per_pass=self.max_views_per_pass,
-                                         fold_layernorm=self.fold_layernorm)
-            else:
-                old = self._packed_version
-                changed = None if old is None else {g for g, key in v.items() if old.get(g) != key}
-                self._engine.load_state_dict(sd, changed=changed)
-            self._packed_version = v
-        return self._engine
+    def _engine_kwargs(self) -> dict:
+        return {"fold_layernorm": bool(self.fold_layernorm)}
 
     @torch.no_grad()
     def embed(self, pixel_values: Tensor) -> Tensor:

@@ -6,14 +6,14 @@ models/clip_embedder.py:26 and evaluation/evaluate.py:36), so checkpoints writte
 """
 from __future__ import annotations
 
-import ctypes as C
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Dict
 
 import torch
 
 from . import _lib
-from ._lib import PigeonB200Error, check, current_stream_ptr, load, ptr
+from ._lib import PigeonB200Error, check, current_stream_ptr, ptr
+from .encoder import EncoderEngine, Pack
 
 
 @dataclass
@@ -45,125 +45,38 @@ class VitDims:
                    ln_eps=float(cfg.layer_norm_eps))
 
 
-def _strip_prefix(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
-    """Normalise HF key names to start at 'embeddings.' / 'encoder.' / 'pre_layrnorm.'."""
-    out = {}
-    for k, v in sd.items():
-        for pre in ("base_model.", "clip_model.", "vision_model."):
-            while k.startswith(pre):
-                k = k[len(pre):]
-        out[k] = v
-    return out
-
-
-class VitEngine:
+class VitEngine(EncoderEngine):
     """H100 execution engine of HF CLIPVisionTransformer.forward(...).last_hidden_state (+ token mean)."""
+    PREFIXES = ("base_model.", "clip_model.", "vision_model.")   # keys start at 'embeddings.' / 'encoder.' / 'pre_layrnorm.'
+    CREATE, DESTROY, WORKSPACE = "pg_vit_create", "pg_vit_destroy", "pg_vit_workspace_bytes"
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], dims: VitDims, device: torch.device | str = "cuda",
                  max_views_per_pass: int = 256, fold_layernorm: bool = True):
         """fold_layernorm: feed the GEMMs the raw fp16 residual row and apply LayerNorm in their epilogues (no LayerNorm
         kernel, no normalised copy in HBM; see csrc/gemm.h EPI_F16_LN_*).  False keeps the LayerNorm kernels (A/B switch)."""
-        self.dims = dims
         self.fold_layernorm = bool(fold_layernorm)
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise PigeonB200Error("VitEngine runs on a CUDA device only (no CPU path)")
         self.max_views_per_pass = int(max_views_per_pass)
-        self._lib = load()
-        self._handle = C.c_void_p()
-        self._ws: Optional[torch.Tensor] = None
-        self._packs = None   # group ("embeddings" | layer index) -> tensors referenced by raw pointer from the C side
-        self.load_state_dict(state_dict)
+        super().__init__(state_dict, dims, device)
 
     # ------------------------------------------------------------------------------------------ weights
-    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], changed=None) -> None:
-        """(Re)pack weights for the kernels.  `changed` limits the work to the groups whose parameters moved: a set holding
-        "embeddings" and / or encoder layer indices (None = everything).  Under the reference's fine-tune policy only the last
-        layer changes between optimizer steps, so one layer is repacked per step instead of 24."""
+    def _pack_embeddings(self, sd: Dict[str, torch.Tensor], pack: Pack) -> tuple:
         d, dev = self.dims, self.device
-        sd = _strip_prefix(state_dict)
-        if changed is None or self._packs is None:
-            changed = {"embeddings", *range(d.layers)}
-            self._packs = {}
-            self._layers = (_lib.VitLayer * d.layers)()
+        pw = sd["embeddings.patch_embedding.weight"].detach().to(dev, torch.float32).reshape(d.hidden, d.patch_k)
+        pw_pad = torch.zeros((d.hidden, d.patch_k_pad), dtype=torch.float32, device=dev)
+        pw_pad[:, : d.patch_k] = pw
+        pos = pack.f32(sd["embeddings.position_embedding.weight"])
+        if pos.shape != (d.tokens, d.hidden):
+            raise PigeonB200Error(f"position_embedding {tuple(pos.shape)} != ({d.tokens}, {d.hidden})")
+        return (ptr(pack.f16(pw_pad)), ptr(pack.f32(sd["embeddings.class_embedding"])), ptr(pos),
+                ptr(pack.f32(sd["pre_layrnorm.weight"])), ptr(pack.f32(sd["pre_layrnorm.bias"])))
 
-        def group(key):
-            keep = []
-            self._packs[key] = keep
-
-            def f32(t):
-                t = t.detach().to(device=dev, dtype=torch.float32).contiguous()
-                keep.append(t)
-                return t
-
-            def f16(t):
-                t = t.detach().to(device=dev, dtype=torch.float32).to(torch.float16).contiguous()
-                keep.append(t)
-                return t
-            return f32, f16
-
-        if "embeddings" in changed:
-            f32, f16 = group("embeddings")
-            pw = sd["embeddings.patch_embedding.weight"].detach().to(dev, torch.float32).reshape(d.hidden, d.patch_k)
-            pw_pad = torch.zeros((d.hidden, d.patch_k_pad), dtype=torch.float32, device=dev)
-            pw_pad[:, : d.patch_k] = pw
-            pos = f32(sd["embeddings.position_embedding.weight"])
-            if pos.shape != (d.tokens, d.hidden):
-                raise PigeonB200Error(f"position_embedding {tuple(pos.shape)} != ({d.tokens}, {d.hidden})")
-            self._top = (ptr(f16(pw_pad)), ptr(f32(sd["embeddings.class_embedding"])), ptr(pos),
-                         ptr(f32(sd["pre_layrnorm.weight"])), ptr(f32(sd["pre_layrnorm.bias"])))
-
-        for i in sorted(k for k in changed if k != "embeddings"):
-            f32, f16 = group(i)
-            p = f"encoder.layers.{i}."
-            w_qkv = torch.cat([sd[p + f"self_attn.{n}_proj.weight"] for n in "qkv"], dim=0)
-            b_qkv = torch.cat([sd[p + f"self_attn.{n}_proj.bias"] for n in "qkv"], dim=0)
-            L = self._layers[i]
-            L.ln1_g, L.ln1_b = ptr(f32(sd[p + "layer_norm1.weight"])), ptr(f32(sd[p + "layer_norm1.bias"]))
-            L.w_qkv, L.b_qkv = ptr(f16(w_qkv)), ptr(f32(b_qkv))
-            L.w_o, L.b_o = ptr(f16(sd[p + "self_attn.out_proj.weight"])), ptr(f32(sd[p + "self_attn.out_proj.bias"]))
-            L.ln2_g, L.ln2_b = ptr(f32(sd[p + "layer_norm2.weight"])), ptr(f32(sd[p + "layer_norm2.bias"]))
-            L.w_fc1, L.b_fc1 = ptr(f16(sd[p + "mlp.fc1.weight"])), ptr(f32(sd[p + "mlp.fc1.bias"]))
-            L.w_fc2, L.b_fc2 = ptr(f16(sd[p + "mlp.fc2.weight"])), ptr(f32(sd[p + "mlp.fc2.bias"]))
-            if self.fold_layernorm:
-                # LN(x) W^T + b = rstd * (x (gamma*W)^T - mu * rowsum(gamma*W)) + (b + W beta): the tensor cores see the raw
-                # row x and W' = gamma * W; rowsum is taken over the fp16 values of W' so that acc - mu * rowsum is exact.
-                def fold(w, b, g, beta):
-                    w32 = w.detach().to(dev, torch.float32)
-                    wf = f16(w32 * g.detach().to(dev, torch.float32)[None, :])
-                    cs = f32(wf.float().sum(dim=1))
-                    bf = f32(b.detach().to(dev, torch.float32) + w32 @ beta.detach().to(dev, torch.float32))
-                    return ptr(wf), ptr(bf), ptr(cs)
-                L.w_qkv_ln, L.b_qkv_ln, L.cs_qkv = fold(w_qkv, b_qkv, sd[p + "layer_norm1.weight"], sd[p + "layer_norm1.bias"])
-                L.w_fc1_ln, L.b_fc1_ln, L.cs_fc1 = fold(sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"],
-                                                         sd[p + "layer_norm2.weight"], sd[p + "layer_norm2.bias"])
-
+    def _structs(self):
+        d = self.dims
         cfg = _lib.VitConfig(d.image_size, d.patch_size, d.hidden, d.heads, d.intermediate, d.layers, d.ln_eps,
                              d.patch_k_pad)
-        w = _lib.VitWeights(*self._top, self._layers)
-        if self._handle:
-            self._lib.pg_vit_destroy(self._handle)
-            self._handle = C.c_void_p()
-        check(self._lib.pg_vit_create(C.byref(cfg), C.byref(w), C.byref(self._handle)), "pg_vit_create")   # copies the structs
-
-    def __del__(self):
-        try:
-            if self._handle:
-                self._lib.pg_vit_destroy(self._handle)
-        except Exception:
-            pass
+        return cfg, _lib.VitWeights(*self._top, self._layers)
 
     # ------------------------------------------------------------------------------------------ forward
-    def workspace_bytes(self, n_views: int) -> int:
-        return int(self._lib.pg_vit_workspace_bytes(self._handle, n_views))
-
-    def _workspace(self, n_views: int) -> torch.Tensor:
-        need = self.workspace_bytes(n_views)
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-        return self._ws
-
     @torch.no_grad()
     def forward(self, pixel_values: torch.Tensor, return_hidden: bool = False):
         """pixel_values [N, 3, H, W] (fp32 or fp16, CUDA) -> token-mean embedding [N, hidden] fp32

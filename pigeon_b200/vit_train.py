@@ -28,6 +28,16 @@ def _aligned_empty(nbytes: int, device) -> torch.Tensor:
     return raw[off:off + nbytes]
 
 
+def grow_aligned(owner, name: str, nbytes: int, device) -> torch.Tensor:
+    """owner.<name>, replaced by a 1024-byte aligned buffer of nbytes when it holds fewer (the old one is freed first)."""
+    buf = getattr(owner, name)
+    if buf is None or buf.numel() < nbytes:
+        setattr(owner, name, None)
+        buf = _aligned_empty(nbytes, device)
+        setattr(owner, name, buf)
+    return buf
+
+
 def put_grad(p, t) -> None:
     """p.grad += t (p.grad = a copy of t when there is none yet): gradient accumulation across backward calls."""
     t = t.contiguous()
@@ -68,6 +78,55 @@ def transpose_layers(layers, versions, wt: list, wt_version: dict) -> None:
         wt[l] = dict(w_qkv_t=wqkv.t().contiguous().to(bf), w_o_t=sa.out_proj.weight.t().contiguous().to(bf),
                      w_fc1_t=mlp.fc1.weight.t().contiguous().to(bf), w_fc2_t=mlp.fc2.weight.t().contiguous().to(bf))
         wt_version[l] = versions[l]
+
+
+def carve_saved(owner, saved, n: int, seq: int, top) -> Dict[str, int]:
+    """Lay the activations a training forward keeps out in owner._arena (grown when too small) for n sequences of seq rows
+    (tokens or S): the tower's `top` entries [(field of `saved`, bytes)] first, then x0 ... h of every encoder layer.  Points
+    `saved` and owner._saved_layers at them and returns the arena offset of each top entry."""
+    d = owner.dims
+    rows, H, I = n * seq, d.hidden, d.intermediate
+    per_layer = [("x0", rows * H * 4), ("xn1", rows * H * 2), ("qkv", rows * 3 * H * 2), ("lse2", n * d.heads * seq * 4),
+                 ("ao", rows * H * 2), ("x1", rows * H * 4), ("xn2", rows * H * 2), ("u", rows * I * 2), ("h", rows * I * 2)]
+    total = sum(_align(b) for _, b in top) + d.layers * sum(_align(b) for _, b in per_layer)
+    base, off, offs = grow_aligned(owner, "_arena", total, next(owner.tower.parameters()).device).data_ptr(), 0, {}
+    if base % 1024:
+        raise PigeonB200Error("activation arena is not 1024-byte aligned")
+    for name, b in top:
+        setattr(saved, name, base + off)
+        offs[name] = off
+        off += _align(b)
+    layers = (_lib.VitSavedLayer * d.layers)()
+    for l in range(d.layers):
+        for name, b in per_layer:
+            setattr(layers[l], name, base + off)
+            off += _align(b)
+    saved.layers_host = owner._saved_layers = layers
+    return offs
+
+
+def flat_grads(shapes, device):
+    """ONE zeroed flat fp32 buffer holding a tensor per (name, shape) of `shapes`, each 16-byte aligned inside it, so a single
+    all-reduce averages them all -> (buffer, {name: view})."""
+    offs, total = [], 0
+    for _, shp in shapes:
+        offs.append(total)
+        total += (int(torch.Size(shp).numel()) + 3) // 4 * 4
+    flat = torch.zeros(total, dtype=torch.float32, device=device)
+    return flat, {name: flat[o:o + int(torch.Size(shp).numel())].view(shp) for (name, shp), o in zip(shapes, offs)}
+
+
+def layers_bwd(wt: list, g: Dict[str, torch.Tensor], trainable) -> C.Array:
+    """The VitLayerBwd array of a backward: every layer's transposed weights, and the gradient buffers of the layers whose
+    `trainable` flag is set."""
+    lb = (_lib.VitLayerBwd * len(wt))()
+    for l, w in enumerate(wt):
+        for k, t in w.items():
+            setattr(lb[l], k, t.data_ptr())
+        if trainable[l]:
+            for k in LAYER_GRADS:
+                setattr(lb[l], "d_" + k, g[f"{l}.{k}"].data_ptr())
+    return lb
 
 
 class TowerTrainer:
@@ -113,32 +172,11 @@ class TowerTrainer:
     def _build_saved(self, n_views: int):
         d = self.dims
         rows = n_views * d.tokens
-        H, I = d.hidden, d.intermediate
-        per_layer = [("x0", rows * H * 4), ("xn1", rows * H * 2), ("qkv", rows * 3 * H * 2),
-                     ("lse2", n_views * d.heads * d.tokens * 4), ("ao", rows * H * 2), ("x1", rows * H * 4),
-                     ("xn2", rows * H * 2), ("u", rows * I * 2), ("h", rows * I * 2)]
-        top = [("im2col", n_views * (d.tokens - 1) * d.patch_k_pad * 2), ("e", rows * H * 4), ("x_out", rows * H * 4)]
-        total = sum(_align(b) for _, b in top) + d.layers * sum(_align(b) for _, b in per_layer)
-        dev = next(self.tower.parameters()).device
-        if self._arena is None or self._arena.numel() < total:
-            self._arena = None
-            self._arena = _aligned_empty(total, dev)
-        base, off = self._arena.data_ptr(), 0
-        if base % 1024:
-            raise PigeonB200Error("activation arena is not 1024-byte aligned")
+        top = [("im2col", n_views * (d.tokens - 1) * d.patch_k_pad * 2), ("e", rows * d.hidden * 4),
+               ("x_out", rows * d.hidden * 4)]
         saved = _lib.VitSaved()
-        for name, b in top:
-            setattr(saved, name, base + off)
-            if name == "x_out":
-                self._x_out_off = off
-            off += _align(b)
-        layers = (_lib.VitSavedLayer * d.layers)()
-        for l in range(d.layers):
-            for name, b in per_layer:
-                setattr(layers[l], name, base + off)
-                off += _align(b)
-        saved.layers_host = layers
-        self._saved, self._saved_layers, self._saved_views = saved, layers, n_views
+        self._x_out_off = carve_saved(self, saved, n_views, d.tokens, top)["x_out"]
+        self._saved, self._saved_views = saved, n_views
 
     def _transposed_weights(self):
         """bf16 transposes of the four weight matrices of every layer (B operands of the backward GEMMs); only the layers whose
@@ -158,21 +196,11 @@ class TowerTrainer:
         if emb_train:
             shapes += [("patch_w", (d.hidden, d.patch_k_pad)), ("class_emb", (d.hidden,)), ("pos_emb", (d.tokens, d.hidden)),
                        ("pre_ln_g", (d.hidden,)), ("pre_ln_b", (d.hidden,))]
-        H, I = d.hidden, d.intermediate
         for l, t in enumerate(layers):
             if t:
-                shapes += layer_grad_shapes(l, H, I)
-        # ONE flat fp32 buffer (every tensor 16-byte aligned inside it): a single all-reduce averages the whole tower
-        offs, total = [], 0
-        for _, shp in shapes:
-            offs.append(total)
-            total += (int(torch.Size(shp).numel()) + 3) // 4 * 4
-        self._pending_flat = torch.zeros(total, dtype=torch.float32, device=dev)
-        g: Dict[str, torch.Tensor] = {}
-        for (name, shp), o in zip(shapes, offs):
-            g[name] = self._pending_flat[o:o + int(torch.Size(shp).numel())].view(shp)
-        self._pending = g
-        return g
+                shapes += layer_grad_shapes(l, d.hidden, d.intermediate)
+        self._pending_flat, self._pending = flat_grads(shapes, dev)
+        return self._pending
 
     # ---------------------------------------------------------------------------------- forward / backward
     @torch.no_grad()
@@ -245,18 +273,11 @@ class TowerTrainer:
         wt = self._transposed_weights()
         g = self._pending_grads()
         emb_train, layers = self.layout()
-        lb = (_lib.VitLayerBwd * d.layers)()
-        for l in range(d.layers):
-            for k, t in wt[l].items():
-                setattr(lb[l], k, t.data_ptr())
-            if layers[l]:
-                for k in LAYER_GRADS:
-                    setattr(lb[l], "d_" + k, g[f"{l}.{k}"].data_ptr())
         grads = _lib.VitGrads()
         if emb_train:
             grads.d_patch_w, grads.d_class_emb, grads.d_pos_emb = g["patch_w"].data_ptr(), g["class_emb"].data_ptr(), g["pos_emb"].data_ptr()
             grads.d_pre_ln_g, grads.d_pre_ln_b = g["pre_ln_g"].data_ptr(), g["pre_ln_b"].data_ptr()
-        grads.layers_host = lb
+        grads.layers_host = layers_bwd(wt, g, layers)
         events, ev_arr = None, None
         if overlap_world > 1:
             if getattr(self, "_bucket_events", None) is None:
@@ -267,12 +288,9 @@ class TowerTrainer:
             events = self._bucket_events
             ev_arr = (C.c_void_p * (d.layers + 1))(*[e.cuda_event for e in events])
             grads.layer_done_events = ev_arr
-        need = int(self._lib.pg_vit_backward_workspace_bytes(eng._handle, n))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = None
-            self._ws = _aligned_empty(need, d_emb.device)
-        check(getattr(self._lib, entry)(eng._handle, C.byref(self._saved), ptr(d_emb), n, C.byref(grads), ptr(self._ws),
-                                        self._ws.numel(), current_stream_ptr()), entry)
+        ws = grow_aligned(self, "_ws", int(self._lib.pg_vit_backward_workspace_bytes(eng._handle, n)), d_emb.device)
+        check(getattr(self._lib, entry)(eng._handle, C.byref(self._saved), ptr(d_emb), n, C.byref(grads), ptr(ws), ws.numel(),
+                                        current_stream_ptr()), entry)
         if overlap_world > 1:
             self._works = []
             with torch.cuda.stream(self._side):
