@@ -179,6 +179,36 @@ int pg_head_loss(const float* logits, int32_t B, int32_t C, int32_t mode, const 
                  double* per_sample, double* loss_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Hierarchical panorama head (reference models/super_guessr.py:94-103,414-433 with panorama=True, hierarchical=True:
+ * models/layers/positional_encoder.py:35-44 then nn.MultiheadAttention(E, heads, dropout, batch_first=True), of whose
+ * output only view 0's row feeds the cell layer).  emb f32 [N, 4, E], E % 16 == 0, E % heads == 0.
+ *   x   = dropout_{p_x}(emb + pe[n0 + n])     sample n of the batch gets positional-encoding row n0 + n on all four views
+ *   q0  = x[:, 0] Wq^T + bq;  k, v = x Wk^T + bk, x Wv^T + bv
+ *   o   = dropout_{p_attn}(softmax(q0 k^T / sqrt(E / heads))) v   per head, over the 4 views
+ *   cls = o Wo^T + bo
+ * Dropout is counter-based (Philox4x32-10 keyed by seed and offset, indexed by the element's position counted from sample
+ * 0 of the whole batch, so chunks n0.. draw what the whole batch draws); p = 0 disables it (evaluation). */
+/* f32 elements of `saved`: x [N*4, E] | q0 [N, E] | kv [N*4, 2E] (k | v) | o [N, E] | probs [N, heads, 4] (before dropout). */
+size_t pg_view_attn_saved_floats(int32_t N, int32_t E, int32_t heads);
+/* Scratch of pg_view_attn_forward and pg_view_attn_backward (either). */
+size_t pg_view_attn_workspace_bytes(int32_t N, int32_t E);
+/* pe f32 [pe_rows, E] (pos_encoder.pos_encoding; n0 + N > pe_rows is refused, as the reference fails past max_len);
+ * w_in3 = pg_head_pack_weight(in_proj_weight [3E, E]) fp16 [3E, 3E], b_in f32 [3E]; w_out3 = pg_head_pack_weight(
+ * out_proj.weight [E, E]) fp16 [E, 3E], b_out f32 [E]  ->  cls f32 [N, E], saved (always written; the backward reads it);
+ * mask_x u8 [N, 4, E] and mask_p u8 [N, heads, 4] (optional, NULL = not written): 1 where dropout kept the element. */
+int pg_view_attn_forward(const float* emb, int32_t N, int32_t E, int32_t heads, const float* pe, int32_t pe_rows,
+                         int32_t n0, const void* w_in3, const float* b_in, const void* w_out3, const float* b_out,
+                         float p_x, float p_attn, uint64_t seed, uint64_t offset, void* workspace, size_t workspace_bytes,
+                         float* saved, uint8_t* mask_x, uint8_t* mask_p, float* cls, void* stream);
+/* Backward in fp32 from dcls f32 [N, E] with the forward's saved, n0, dropout probabilities, seed and offset (the masks are
+ * regenerated): dw_in f32 [3E, E], db_in [3E], dw_out [E, E], db_out [E] (each may be NULL; `accumulate` != 0 adds into
+ * them) and demb f32 [N, 4, E] (written).  w_in / w_out are the f32 in_proj_weight / out_proj.weight. */
+int pg_view_attn_backward(const float* dcls, int32_t N, int32_t E, int32_t heads, int32_t n0, const float* w_in,
+                          const float* w_out, const float* saved, float p_x, float p_attn, uint64_t seed, uint64_t offset,
+                          int32_t accumulate, float* dw_in, float* db_in, float* dw_out, float* db_out, float* demb,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * Image pre-processing ("next" row N2): what `CLIPProcessor.from_pretrained(CLIP_MODEL)(images=...)` does on the
  * CPU per item in reference dataset_creation/finetune/embed_dataset.py:17-22, preprocessing/dataset_preprocessing.py:
  * 182-204, dataset_creation/benchmark/benchmark_dataset.py:100-104 (transformers 4.23.1 CLIPFeatureExtractor over

@@ -30,6 +30,7 @@ SOURCES = [
     "vit_misc.cu",
     "head.cu",
     "head_fused_wgmma.cu",
+    "view_attention.cu",
     "refiner.cu",
     "train.cu",
     "preprocess.cu",

@@ -185,6 +185,14 @@ SIGNATURES = {
                                   c_void_p, c_void_p]),
     "pg_head_loss": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_double,
                                c_void_p, c_void_p, c_void_p]),
+    "pg_view_attn_saved_floats": (c_size_t, [c_int32, c_int32, c_int32]),
+    "pg_view_attn_workspace_bytes": (c_size_t, [c_int32, c_int32]),
+    "pg_view_attn_forward": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_float, c_float, C.c_uint64, C.c_uint64, c_void_p, c_size_t,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pg_view_attn_backward": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_float,
+                                        c_float, C.c_uint64, C.c_uint64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_size_t, c_void_p]),
     "pg_preprocess_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
     "pg_preprocess_clip": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int32,
                                      c_void_p]),

@@ -339,6 +339,67 @@ def head_forward(emb: torch.Tensor, w3: torch.Tensor, bias: torch.Tensor, centro
     return out
 
 
+def view_attention_forward(emb: torch.Tensor, pe: torch.Tensor, w_in3: torch.Tensor, b_in: torch.Tensor,
+                           w_out3: torch.Tensor, b_out: torch.Tensor, heads: int = 16, n0: int = 0, p_x: float = 0.0,
+                           p_attn: float = 0.0, seed: int = 0, offset: int = 0, return_masks: bool = False) -> dict:
+    """The hierarchical head's view self-attention (pg_view_attn_forward): emb f32 [N, 4, E], pe = pos_encoder.pos_encoding
+    f32 [rows, 1, E] (sample n uses row n0 + n), in_proj / out_proj packed by `head_pack_weight` -> dict(cls f32 [N, E],
+    saved f32 (what `view_attention_backward` reads; `view_attention_saved` names its parts)) and, with `return_masks`,
+    mask_x bool [N, 4, E] and mask_p bool [N, heads, 4]: where the two dropouts kept the element."""
+    _need_cuda(emb, pe, w_in3, b_in, w_out3, b_out)
+    if emb.dtype != torch.float32 or emb.dim() != 3 or emb.shape[1] != 4:
+        raise PigeonB200Error(f"view attention needs f32 embeddings [N, 4, E], got {emb.dtype} {tuple(emb.shape)}")
+    N, _, E = emb.shape
+    if pe.shape[-1] != E or w_in3.shape != (3 * E, 3 * E) or w_out3.shape != (E, 3 * E):
+        raise PigeonB200Error(f"view attention weights {tuple(w_in3.shape)}, {tuple(w_out3.shape)} or positional encoding "
+                              f"{tuple(pe.shape)} do not match E = {E}")
+    lib = load()
+    dev = emb.device
+    saved = torch.empty(max(1, lib.pg_view_attn_saved_floats(N, E, heads)), dtype=torch.float32, device=dev)
+    ws = torch.empty(max(1, lib.pg_view_attn_workspace_bytes(N, E)), dtype=torch.uint8, device=dev)
+    cls = torch.empty((N, E), dtype=torch.float32, device=dev)
+    mask_x = torch.empty((N, 4, E), dtype=torch.uint8, device=dev) if return_masks else None
+    mask_p = torch.empty((N, heads, 4), dtype=torch.uint8, device=dev) if return_masks else None
+    check(lib.pg_view_attn_forward(ptr(emb), N, E, heads, ptr(pe), pe.shape[0], n0, ptr(w_in3), ptr(b_in), ptr(w_out3),
+                                   ptr(b_out), float(p_x), float(p_attn), int(seed), int(offset), ptr(ws), ws.numel(),
+                                   ptr(saved), ptr(mask_x), ptr(mask_p), ptr(cls), current_stream_ptr()),
+          "pg_view_attn_forward")
+    out = dict(cls=cls, saved=saved)
+    if return_masks:
+        out.update(mask_x=mask_x.bool(), mask_p=mask_p.bool())
+    return out
+
+
+def view_attention_saved(saved: torch.Tensor, N: int, E: int, heads: int = 16) -> dict:
+    """Named views of `view_attention_forward`'s saved activations: x [N, 4, E] (after the positional encoding and its
+    dropout), q0 [N, E], k [N, 4, E], v [N, 4, E], o [N, E] (attention output before out_proj), probs [N, heads, 4]."""
+    ne = N * E
+    kv = saved[5 * ne:13 * ne].view(N, 4, 2 * E)
+    return dict(x=saved[:4 * ne].view(N, 4, E), q0=saved[4 * ne:5 * ne].view(N, E), k=kv[..., :E], v=kv[..., E:],
+                o=saved[13 * ne:14 * ne].view(N, E), probs=saved[14 * ne:14 * ne + 4 * N * heads].view(N, heads, 4))
+
+
+def view_attention_backward(dcls: torch.Tensor, saved: torch.Tensor, w_in: torch.Tensor, w_out: torch.Tensor,
+                            heads: int = 16, n0: int = 0, p_x: float = 0.0, p_attn: float = 0.0, seed: int = 0,
+                            offset: int = 0, grads=None, accumulate: bool = False) -> torch.Tensor:
+    """Backward of `view_attention_forward` (same n0, dropout probabilities, seed and offset): dcls f32 [N, E] -> d emb
+    f32 [N, 4, E].  `grads` = (d in_proj_weight [3E, E], d in_proj_bias [3E], d out_proj.weight [E, E], d out_proj.bias [E])
+    f32 tensors written, or added into with `accumulate` (entries may be None)."""
+    dcls = dcls.to(torch.float32).contiguous()
+    w_in, w_out = w_in.detach().contiguous(), w_out.detach().contiguous()
+    grads = tuple(grads) if grads is not None else (None,) * 4
+    _need_cuda(dcls, saved, w_in, w_out, *grads)
+    N, E = dcls.shape
+    lib = load()
+    dev = dcls.device
+    ws = torch.empty(max(1, lib.pg_view_attn_workspace_bytes(N, E)), dtype=torch.uint8, device=dev)
+    demb = torch.empty((N, 4, E), dtype=torch.float32, device=dev)
+    check(lib.pg_view_attn_backward(ptr(dcls), N, E, heads, n0, ptr(w_in), ptr(w_out), ptr(saved), float(p_x),
+                                    float(p_attn), int(seed), int(offset), int(bool(accumulate)), *(ptr(g) for g in grads),
+                                    ptr(demb), ptr(ws), ws.numel(), current_stream_ptr()), "pg_view_attn_backward")
+    return demb
+
+
 class DeviceBank:
     """CSR prototype bank resident in HBM (layout of `pg_refiner_bank`, include/pigeon_b200.h)."""
 

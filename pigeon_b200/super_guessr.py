@@ -8,6 +8,7 @@ of libpigeon_b200.so; there is no PyTorch/CPU fallback for it.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from types import SimpleNamespace
 from typing import Optional
 
@@ -30,6 +31,24 @@ NUM_CLIMATES = 28
 CLIMATE_LOSS_SCALING = 2
 NUM_MONTHS = 12
 MONTHS_LOSS_SCALING = 1
+NUM_ATTENTION_HEADS = 16
+
+
+class PositionalEncoder(nn.Module):
+    """reference models/layers/positional_encoder.py: the sinusoidal table of the PyTorch transformer tutorial,
+    pos_encoding [max_len, 1, dim] (a Parameter without gradient, so checkpoints carry it), and the dropout after the add.
+    Its forward runs inside pg_view_attn_forward, where sample n of the batch gets row n on all four views, as the
+    reference's `pos_encoding[:token_embedding.size(0)]` with batch_first inputs does."""
+
+    def __init__(self, dim_model: int, dropout_p: float = 0.1, max_len: int = 1000):
+        super().__init__()
+        self.dropout = nn.Dropout(dropout_p)
+        positions = torch.arange(0, max_len, dtype=torch.float).view(-1, 1)
+        division = torch.exp(torch.arange(0, dim_model, 2).float() * (-math.log(10000.0)) / dim_model)
+        table = torch.zeros(max_len, dim_model)
+        table[:, 0::2] = torch.sin(positions * division)
+        table[:, 1::2] = torch.cos(positions * division)
+        self.pos_encoding = Parameter(table.unsqueeze(1), requires_grad=False)
 
 
 class CLIPVisionTower(EncoderTower, nn.Module):
@@ -121,11 +140,12 @@ class SuperGuessr(nn.Module):
         geocells = kwargs.pop("geocells", None)
         if len(kwargs) > 0:
             print(f'Not using keyword arguments: {list(kwargs.keys())}')  # :67-68
-        if hierarchical:
-            raise NotImplementedError("hierarchical=True (experimental self-attention pooling, disabled in the shipped "
-                                      "configs: evaluate.py:42, train_modes.py:99,126) is outside the H100 hot path")
         if heading and not panorama:
             raise NotImplementedError("heading features for single images are outside the H100 hot path")
+        if hierarchical and heading:
+            raise NotImplementedError("hierarchical=True with heading=True: the reference pads the attention width to "
+                                      "input_dim + 14 and its cell layer then rejects the wider CLS row "
+                                      "(super_guessr.py:90-98,420-433)")
 
         self.base_model = as_tower(base_model)
         self.panorama = panorama
@@ -149,6 +169,11 @@ class SuperGuessr(nn.Module):
         self.num_cells = self.lla_geocells.size(0)
         self.input_dim = self.hidden_size   # panorama + heading leaves the input unchanged (:279-280)
 
+        if self.hierarchical:                                                   # :94-103
+            print('Number of attention heads:', NUM_ATTENTION_HEADS)
+            self.pos_encoder = PositionalEncoder(self.input_dim)
+            self.self_attn = nn.MultiheadAttention(self.input_dim, NUM_ATTENTION_HEADS, dropout=0.1, batch_first=True)
+            self.relu = nn.ReLU()
         self.cell_layer = nn.Linear(self.input_dim, self.num_cells)
         self.softmax = nn.Softmax(dim=-1)
         if self.multi_task:
@@ -164,6 +189,8 @@ class SuperGuessr(nn.Module):
         self.loss_fnc = nn.CrossEntropyLoss()
         self._w3 = None
         self._w3_key = None
+        self._attn_packs = {}
+        self._attn_state = None
         self.last_pooled = None
         print(f'Initialized SuperGuessr classification model with {self.num_cells} geocells.')
 
@@ -231,6 +258,53 @@ class SuperGuessr(nn.Module):
             self._w3_key = key
         return self._w3
 
+    # ---------------------------------------------------------------------------------- hierarchical head (:94-103, :414-433)
+    def _hierarchical(self) -> bool:
+        return self.hierarchical and self.panorama
+
+    def _packed_attn(self):
+        """fp16 split copies of in_proj_weight and out_proj.weight, repacked whenever the weights change (same key as
+        `_packed_head`: torch's version counter plus the raw-pointer updates the optimizers record)."""
+        out = []
+        for w in (self.self_attn.in_proj_weight, self.self_attn.out_proj.weight):
+            key = (w.data_ptr(), w._version, _versions.get(w))
+            hit = self._attn_packs.get(id(w))
+            if hit is None or hit[0] != key:
+                hit = self._attn_packs[id(w)] = (key, ops.head_pack_weight(w.detach()))
+            out.append(hit[1])
+        return out
+
+    def _attn_params(self):
+        sa = self.self_attn
+        return [sa.in_proj_weight, sa.in_proj_bias, sa.out_proj.weight, sa.out_proj.bias]
+
+    def _draw_dropout_rng(self):
+        """(seed, offset) of this forward's dropout masks, drawn once from torch's default generator in training mode, so
+        torch.manual_seed reproduces a run; evaluation draws nothing (no dropout)."""
+        if not self.training:
+            return 0, 0
+        seed, offset = torch.randint(0, 2 ** 62, (2,)).tolist()
+        return seed, offset
+
+    def _attn_forward(self, emb: Tensor, n0: int, rng) -> Tensor:
+        """View self-attention of the panorama emb f32 [n, 4, E] (samples n0.. of the batch) -> the CLS row f32 [n, E];
+        keeps what the backward needs in `self._attn_state`."""
+        sa = self.self_attn
+        p_x, p_attn = (float(self.pos_encoder.dropout.p), float(sa.dropout)) if self.training else (0.0, 0.0)
+        w_in3, w_out3 = self._packed_attn()
+        a = ops.view_attention_forward(emb, self.pos_encoder.pos_encoding.data, w_in3,
+                                       sa.in_proj_bias.detach().float().contiguous(), w_out3,
+                                       sa.out_proj.bias.detach().float().contiguous(), NUM_ATTENTION_HEADS, n0, p_x, p_attn,
+                                       *rng)
+        self._attn_state = dict(saved=a["saved"], n0=n0, p_x=p_x, p_attn=p_attn, seed=rng[0], offset=rng[1])
+        return a["cls"]
+
+    def _attn_backward(self, dcls: Tensor, grads, accumulate: bool) -> Tensor:
+        st = self._attn_state
+        return ops.view_attention_backward(dcls, st["saved"], self.self_attn.in_proj_weight, self.self_attn.out_proj.weight,
+                                           NUM_ATTENTION_HEADS, st["n0"], st["p_x"], st["p_attn"], st["seed"], st["offset"],
+                                           grads=grads, accumulate=accumulate)
+
     def _classification_loss(self, logits: Tensor, labels: Optional[Tensor], labels_clf: Tensor,
                              want_grad: bool = False, grad_scale: float = 1.0) -> Tensor:
         """reference :456,468-474 on the GPU (pg_head_loss); with `want_grad` also d loss / d logits (pg_head_loss_grad),
@@ -293,7 +367,12 @@ class SuperGuessr(nn.Module):
         w, b = self.cell_layer.weight, self.cell_layer.bias
         Cc, D = w.shape
         head_trains = w.requires_grad
-        flat = torch.zeros(Cc * D + Cc, dtype=torch.float32, device=dev)
+        hier = self._hierarchical()
+        # the self_attn gradients ride in the head's flat buffer, so one all-reduce averages both
+        attn_sizes = [p.numel() for p in self._attn_params()] if hier else []
+        flat = torch.zeros(Cc * D + Cc + sum(attn_sizes), dtype=torch.float32, device=dev)
+        attn_grads = list(torch.split(flat[Cc * D + Cc:], attn_sizes)) if hier else None
+        rng = self._draw_dropout_rng() if hier else None
         lib = load()
         from . import dist as pdist
         pdist_world = pdist.world_size()
@@ -304,7 +383,9 @@ class SuperGuessr(nn.Module):
                 hi = min(B, lo + step)
                 n = hi - lo
                 emb = tr.forward(px[lo * V:hi * V].to(dev, non_blocking=True)).reshape(n, V, D)
-                h = ops.head_forward(emb.contiguous(), self._packed_head(), b.detach().float().contiguous(),
+                # the PE row of a sample is its index in the whole batch (lo + i), so chunks see what the whole batch sees
+                head_in = self._attn_forward(emb.contiguous(), lo, rng).unsqueeze(1) if hier else emb.contiguous()
+                h = ops.head_forward(head_in, self._packed_head(), b.detach().float().contiguous(),
                                      self.lla_geocells.data, self.num_candidates)
                 loss = self._classification_loss(h["logits"], None if labels is None else labels[lo:hi], labels_clf[lo:hi],
                                                  want_grad=True, grad_scale=n / B)
@@ -322,7 +403,10 @@ class SuperGuessr(nn.Module):
                         mt_loss[i] = mt_loss[i] + mt[3 + i] * (n / B)
                     dpooled += mt[6]
                     mt_grads = mt[7] if mt_grads is None else [a + b_ for a, b_ in zip(mt_grads, mt[7])]
-                d_emb = (dpooled / V).repeat_interleave(V, dim=0) if V > 1 else dpooled      # backward of the view mean
+                if hier:                                                                  # backward of the view attention
+                    d_emb = self._attn_backward(dpooled, attn_grads, accumulate=True).reshape(n * V, D)
+                else:
+                    d_emb = (dpooled / V).repeat_interleave(V, dim=0) if V > 1 else dpooled  # backward of the view mean
                 # last chunk under torch.distributed: the gradient all-reduce rides behind this backward, bucket by bucket
                 tr.backward(d_emb, overlap_world=pdist_world if hi == B else 1)
                 part = loss.double() * (n / B)
@@ -333,7 +417,9 @@ class SuperGuessr(nn.Module):
         cat = lambda k: torch.cat([h[k] for h, _ in outs])
         embedding = torch.cat([e for _, e in outs])
         loss_clf = loss_total if self.should_smooth_labels else loss_total.to(torch.float32)
-        self.last_pooled = cat("pooled")
+        # what the refiner gets: the view mean, or None when the head read the attention's CLS row (the refiner then
+        # averages the raw views itself, proto_refiner.py:138-139)
+        self.last_pooled = None if hier else cat("pooled")
         preds_mt = preds_climate = preds_month = None
         loss = loss_clf
         if self.multi_task:
@@ -361,18 +447,23 @@ class SuperGuessr(nn.Module):
             Cc, D = w.shape
             if w.requires_grad:
                 if w.grad is None:
-                    w.grad, b.grad = flat[: Cc * D].view(Cc, D), flat[Cc * D:]
+                    w.grad, b.grad = flat[: Cc * D].view(Cc, D), flat[Cc * D:Cc * D + Cc]
                 else:
                     w.grad.add_(flat[: Cc * D].view(Cc, D))
-                    b.grad.add_(flat[Cc * D:])
+                    b.grad.add_(flat[Cc * D:Cc * D + Cc])
+            if self._hierarchical():
+                self._publish_attn_grads(flat[Cc * D + Cc:])
             self._trainer.finalize(world)
             self._publish_mt_grads(getattr(self, "_pend_mt", None), world)
             self._pend_mt = None
             return
-        if getattr(self, "_saved_dlogits", None) is None or self.last_pooled is None:
+        if getattr(self, "_saved_dlogits", None) is None or getattr(self, "_head_in", None) is None:
             raise PigeonB200Error("backward() needs a preceding training-mode forward with labels")
+        if self._hierarchical():
+            self._backward_hierarchical(grad_scale)
+            return
         w, b = self.cell_layer.weight, self.cell_layer.bias
-        dlog, pooled = self._saved_dlogits, self.last_pooled
+        dlog, pooled = self._saved_dlogits, self._head_in
         B, Cc = dlog.shape
         D = pooled.shape[1]
         if grad_scale != 1.0:
@@ -400,6 +491,44 @@ class SuperGuessr(nn.Module):
         self._saved_dlogits = None
         self._publish_mt_grads(getattr(self, "_saved_mt", None), world)
         self._saved_mt = None
+
+    def _backward_hierarchical(self, grad_scale: float) -> None:
+        """backward() of the hierarchical head on embeddings: cell_layer, the auxiliary heads' d output, then the view
+        attention; the cell_layer and self_attn gradients share one flat buffer (one all-reduce under torch.distributed)."""
+        from . import dist as pdist
+        w, b = self.cell_layer.weight, self.cell_layer.bias
+        dlog, cls = self._saved_dlogits, self._head_in
+        if grad_scale != 1.0:
+            dlog = dlog * grad_scale
+        B, Cc = dlog.shape
+        D = cls.shape[1]
+        sizes = [Cc * D, Cc] + [p.numel() for p in self._attn_params()]
+        flat = torch.empty(sum(sizes), dtype=torch.float32, device=dlog.device)
+        gw, gb, *attn_grads = torch.split(flat, sizes)
+        dcls = torch.empty((B, D), dtype=torch.float32, device=dlog.device)
+        check(load().pg_head_backward(ptr(dlog), ptr(cls), ptr(w.detach()), B, Cc, D, 0, ptr(gw), ptr(gb), ptr(dcls),
+                                      current_stream_ptr()), "pg_head_backward")
+        if self._saved_mt_dx is not None:
+            dcls += self._saved_mt_dx * grad_scale
+        self._attn_backward(dcls, attn_grads, accumulate=False)
+        world = pdist.world_size()
+        if world > 1:
+            torch.distributed.all_reduce(flat)
+            flat.mul_(1.0 / world)
+        if w.requires_grad:
+            w.grad = gw.view(Cc, D).clone() if w.grad is None else w.grad.add_(gw.view(Cc, D))
+            b.grad = gb.clone() if b.grad is None else b.grad.add_(gb)
+        self._publish_attn_grads(flat[Cc * D + Cc:])
+        self._saved_dlogits = None
+        self._saved_mt_dx = None
+        self._publish_mt_grads(getattr(self, "_saved_mt", None), world)
+        self._saved_mt = None
+
+    def _publish_attn_grads(self, flat: Tensor) -> None:
+        """Accumulates the (already averaged) self_attn gradients held in `flat` into `.grad`."""
+        for p, g in zip(self._attn_params(), torch.split(flat, [p.numel() for p in self._attn_params()])):
+            if p.requires_grad:
+                p.grad = g.view_as(p).clone() if p.grad is None else p.grad.add_(g.view_as(p))
 
     # ---------------------------------------------------------------------------------- multi-task heads (:315-348)
     _MT_HEADS = ("multi_task_head", "climate_layer", "month_layer")
@@ -456,7 +585,7 @@ class SuperGuessr(nn.Module):
         if want_grad:
             tower_trains = self.base_model is not None and any(p.requires_grad for p in self.base_model.parameters())
             stray = [n for n in self._trainable_outside_head()
-                     if not n.startswith("base_model.") and n.split(".")[0] not in self._MT_HEADS]
+                     if not n.startswith("base_model.") and n.split(".")[0] not in self._MT_HEADS + ("self_attn",)]
             if stray:
                 raise NotImplementedError(f"no backward for trainable parameters {stray[:3]}")
             if tower_trains:
@@ -490,21 +619,29 @@ class SuperGuessr(nn.Module):
             else:
                 head_in = layer_input.unsqueeze(1) if layer_input.dim() == 2 else layer_input
             head_in = head_in.contiguous()
+            hier = self._hierarchical()
+            if hier:                                                            # :414-433, CLS row of view 0
+                head_in = self._attn_forward(head_in, 0, self._draw_dropout_rng()).unsqueeze(1)
 
             h = ops.head_forward(head_in, self._packed_head(), self.cell_layer.bias.detach().float().contiguous(),
                                  self.lla_geocells.data, self.num_candidates)   # :447-459
             output, logits = h["pooled"], h["logits"]
-            self.last_pooled = output           # extension: view-averaged embedding, reused by evaluation.predict_batch
+            self._head_in = output
+            # extension: view-averaged embedding, reused by evaluation.predict_batch as the refiner's input; the hierarchical
+            # head's CLS row is not what the refiner reads (proto_refiner.py:138-139 averages the raw views)
+            self.last_pooled = None if hier else output
             pred_LLH, geocell_preds = h["pred_lnglat"], h["pred_cell"]
             geocell_topk = TopK(h["topk_val"], h["topk_idx"])
 
             preds_mt = preds_climate = preds_month = None
             loss_reg = loss_climate = loss_month = 0
             self._saved_mt = None
+            self._saved_mt_dx = None
             if self.multi_task:                                                 # :315-348
-                (preds_mt, preds_climate, preds_month, loss_reg, loss_climate, loss_month, _, mt_grads) = self._multi_task(
+                (preds_mt, preds_climate, preds_month, loss_reg, loss_climate, loss_month, mt_dx, mt_grads) = self._multi_task(
                     output, labels_multi_task, labels_climate, labels_month, dev, want_grad)
                 self._saved_mt = mt_grads
+                self._saved_mt_dx = mt_dx
 
             if not self.training and self.serving:                              # :462-466
                 if self.multi_task:
