@@ -225,6 +225,21 @@ size_t pg_preprocess_workspace_bytes(const pg_image* images, int32_t n, int32_t 
 /* out: [n, 3, size, size] f32 (out_f16 = 0) or f16 (out_f16 = 1, round-to-nearest of the f32 value); mean/std: host float[3]. */
 int pg_preprocess_clip(const pg_image* images, int32_t n, int32_t size, const float* mean, const float* std,
                        void* workspace, size_t workspace_bytes, void* out, int32_t out_f16, void* stream);
+/* The same with each image first cut to a source rectangle, which may extend past the image: what torchvision's
+ * CenterCrop (padding with 0 in the file's mode) or a Pillow crop box does before CLIPProcessor in reference
+ * dataset_creation/pretrain/pretrain_dataset.py:109-161 and pretrain_dataset_yfcc.py:154-173.  windows[i] is a HOST
+ * descriptor in image i's pixel coordinates; samples outside the image read `fill` (RGB).  The rectangle then stands in
+ * for the image: its shortest edge is resized to `size` and centre-cropped.  width * 3 <= 96 KiB.  n may exceed 65535. */
+typedef struct pg_window {
+  int32_t x0, y0;       /* top-left corner; negative = left of / above the image */
+  int32_t width, height;
+  uint8_t fill[3];
+  uint8_t reserved;
+} pg_window;
+size_t pg_preprocess_window_workspace_bytes(const pg_image* images, const pg_window* windows, int32_t n, int32_t size);
+int pg_preprocess_clip_window(const pg_image* images, const pg_window* windows, int32_t n, int32_t size,
+                              const float* mean, const float* std, void* workspace, size_t workspace_bytes, void* out,
+                              int32_t out_f16, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Baseline JPEG decoding (csrc/jpeg.cu): what `PIL.Image.open(f).convert('RGB')` does on the CPU before every

@@ -27,6 +27,11 @@ class Image(C.Structure):
     _fields_ = [("data", c_void_p), ("height", c_int32), ("width", c_int32), ("row_stride", c_int64)]
 
 
+class Window(C.Structure):
+    _fields_ = [("x0", c_int32), ("y0", c_int32), ("width", c_int32), ("height", c_int32), ("fill", C.c_uint8 * 3),
+                ("reserved", C.c_uint8)]
+
+
 class VitLayer(C.Structure):
     _fields_ = [(n, c_void_p) for n in ("ln1_g", "ln1_b", "w_qkv", "b_qkv", "w_o", "b_o", "ln2_g", "ln2_b",
                                         "w_fc1", "b_fc1", "w_fc2", "b_fc2", "w_qkv_ln", "b_qkv_ln", "cs_qkv",
@@ -196,6 +201,9 @@ SIGNATURES = {
     "pg_preprocess_workspace_bytes": (c_size_t, [c_void_p, c_int32, c_int32]),
     "pg_preprocess_clip": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int32,
                                      c_void_p]),
+    "pg_preprocess_window_workspace_bytes": (c_size_t, [c_void_p, c_void_p, c_int32, c_int32]),
+    "pg_preprocess_clip_window": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_size_t,
+                                            c_void_p, c_int32, c_void_p]),
     "pg_jpeg_parse": (c_int32, [c_void_p, c_int64, C.POINTER(JpegInfo)]),
     "pg_jpeg_parse_multiscan": (c_int32, [c_void_p, c_int64, C.POINTER(JpegInfo)]),
     "pg_jpeg_scans": (c_int32, [c_void_p, c_int64, C.POINTER(JpegScan), c_int32]),

@@ -6,6 +6,16 @@ from types import SimpleNamespace
 CLIP_MODEL = 'openai/clip-vit-large-patch14-336'
 CLIP_EMBED_DIM = 1024
 
+# Pretraining data: metadata CSVs, image folders and the CLIP tokenizer   (config.py:11-19, 49)
+PRETRAIN_METADATA_PATH = 'data/data_pretrain.csv'
+IMAGE_PATH = 'data/streetview_outputs_cropped'
+IMAGE_PATH_2 = 'data/streetview_part_2_data'
+PRETRAIN_METADATA_PATH_YFCC = 'data/data_yfcc_augmented_non_contaminated.csv'
+IMAGE_PATH_YFCC = 'data/images_mp_16/jpgs'
+DRIVING_SIDE_PATH = 'data/driving_side/countries_driving_side.json'
+# A local copy of CLIP_MODEL's tokenizer files (vocab.json, merges.txt): nothing is downloaded
+CLIP_TOKENIZER_PATH = 'saved_models/clip_tokenizer'
+
 # Geocells path                                                        (config.py:34-36)
 GEOCELL_PATH = 'data/geocells_2203.csv'       # PIGEON
 GEOCELL_PATH_YFCC = 'data/geocells_yfcc.csv'  # PIGEOTTO

@@ -292,12 +292,25 @@ int pg_head_loss(const float* logits, int32_t B, int32_t C, int32_t mode, const 
 }
 
 size_t pg_preprocess_workspace_bytes(const pg_image* images, int32_t n, int32_t size) {
-  return preprocess_workspace_bytes(images, n, size);
+  return preprocess_workspace_bytes(images, nullptr, n, size);
 }
 
 int pg_preprocess_clip(const pg_image* images, int32_t n, int32_t size, const float* mean, const float* stdv,
                        void* workspace, size_t workspace_bytes, void* out, int32_t out_f16, void* stream) {
-  return preprocess_clip(images, n, size, mean, stdv, workspace, workspace_bytes, out, out_f16,
+  return preprocess_clip(images, nullptr, n, size, mean, stdv, workspace, workspace_bytes, out, out_f16,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+size_t pg_preprocess_window_workspace_bytes(const pg_image* images, const pg_window* windows, int32_t n, int32_t size) {
+  if (!windows) { set_last_error("pg_preprocess_window_workspace_bytes: windows is NULL"); return 0; }
+  return preprocess_workspace_bytes(images, windows, n, size);
+}
+
+int pg_preprocess_clip_window(const pg_image* images, const pg_window* windows, int32_t n, int32_t size,
+                              const float* mean, const float* stdv, void* workspace, size_t workspace_bytes, void* out,
+                              int32_t out_f16, void* stream) {
+  if (!windows) { set_last_error("pg_preprocess_clip_window: windows is NULL"); return 1; }
+  return preprocess_clip(images, windows, n, size, mean, stdv, workspace, workspace_bytes, out, out_f16,
                          reinterpret_cast<cudaStream_t>(stream));
 }
 

@@ -16,11 +16,16 @@ least as fast as the host route on progressive photos; DESIGN.md §1).  `png=Tru
 so pixels and exceptions are those of the default route either way.
 `square_crop=True` (a keyword of the call) first cuts every decoded image to its centred square, the reference's
 `BenchmarkDataset._crop_images` (benchmark_dataset.py:52-66): a strided view of a device image, a slice of a host one.
+`windows=[CropWindow, ...]` (with `fills`) cuts each image to a rectangle that may extend past it, the crops of the
+reference's pretraining datasets (pigeon_b200.pretrain_data): `pg_preprocess_clip_window` reads the fill colour for
+samples outside the image, so nothing is padded in memory.  The same file object given several times in one call is
+decoded once.
 """
 from __future__ import annotations
 
+import ctypes as C
 import io
-from typing import List, Sequence, Union
+from typing import List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -57,6 +62,35 @@ def _square(img):
     """Centred square view of an [H, W, 3] array or tensor (rows keep their stride, pixels stay contiguous)."""
     h0, w0, s = square_crop_box(img.shape[0], img.shape[1])
     return img[h0:h0 + s, w0:w0 + s]
+
+
+class CropWindow(NamedTuple):
+    """The rectangle of an image that pre-processing reads: `x0, y0, width, height` in pixels, relative to the image or,
+    with `clip = (left, top, width, height)`, to that part of it, cut first as a numpy slice does (clamped to the
+    image).  The rectangle may extend past the image (or past `clip`); samples there take the call's fill colour."""
+    x0: int
+    y0: int
+    width: int
+    height: int
+    clip: Optional[Tuple[int, int, int, int]] = None
+
+
+def _clip(img, window: CropWindow):
+    """`img[top:top + h, left:left + w]` of the window's clip (a view), or `img` without one."""
+    if window.clip is None:
+        return img
+    left, top, w, h = window.clip
+    return img[top:top + h, left:left + w]
+
+
+def _host_window(img, window: CropWindow) -> np.ndarray:
+    """Pillow's crop of a PIL image for a window whose padding is not one RGB colour: clip, then `Image.crop` (which
+    fills outside the image with 0 in the image's mode, as torchvision's pad does), then `convert('RGB')`."""
+    if window.clip is not None:
+        left, top, w, h = window.clip
+        img = img.crop((min(left, img.width), min(top, img.height), min(left + w, img.width), min(top + h, img.height)))
+    img = img.crop((window.x0, window.y0, window.x0 + window.width, window.y0 + window.height))
+    return _to_u8_rgb(img)
 
 
 def route_encoded(data, multiscan: bool = False, png: bool = False) -> tuple:
@@ -103,30 +137,93 @@ class ClipImageProcessor:
         self.gpu_decoded = 0
         self.host_decoded = 0
 
-    def preprocess_device(self, images_u8: List[torch.Tensor]) -> torch.Tensor:
-        """images_u8: CUDA uint8 tensors [H, W, 3] (any sizes, rows may be strided) -> [n, 3, size, size]."""
+    def preprocess_device(self, images_u8: List[torch.Tensor], windows: Optional[Sequence[tuple]] = None) -> torch.Tensor:
+        """images_u8: CUDA uint8 tensors [H, W, 3] (any sizes, rows may be strided) -> [n, 3, size, size].  `windows`:
+        one (x0, y0, width, height, (r, g, b) fill) per image, the source rectangle of `pg_preprocess_clip_window`."""
         n = len(images_u8)
         desc = (_lib.Image * n)()
         for i, t in enumerate(images_u8):
             if not t.is_cuda or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3 or t.stride(2) != 1 or t.stride(1) != 3:
                 raise ValueError("images must be CUDA uint8 [H, W, 3] tensors with contiguous pixels")
             desc[i] = _lib.Image(t.data_ptr(), t.shape[0], t.shape[1], t.stride(0))
-        need = int(self._lib.pg_preprocess_workspace_bytes(desc, n, self.size))
+        win = None
+        if windows is not None:
+            if len(windows) != n:
+                raise ValueError(f"{len(windows)} windows for {n} images")
+            win = (_lib.Window * n)()
+            for i, (x0, y0, w, h, fill) in enumerate(windows):
+                win[i] = _lib.Window(int(x0), int(y0), int(w), int(h), (C.c_uint8 * 3)(*(int(c) for c in fill)), 0)
+            need = int(self._lib.pg_preprocess_window_workspace_bytes(desc, win, n, self.size))
+        else:
+            need = int(self._lib.pg_preprocess_workspace_bytes(desc, n, self.size))
         if need == 0:
             raise PigeonB200Error(f"pg_preprocess_workspace_bytes: {self._lib.pg_last_error().decode()}")
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         out = torch.empty((n, 3, self.size, self.size), dtype=self.dtype, device=self.device)
+        if win is not None:
+            check(self._lib.pg_preprocess_clip_window(desc, win, n, self.size, self.mean.ctypes.data, self.std.ctypes.data,
+                                                      self._ws.data_ptr(), self._ws.numel(), out.data_ptr(),
+                                                      int(self.dtype == torch.float16), current_stream_ptr()),
+                  "pg_preprocess_clip_window")
+            return out
         check(self._lib.pg_preprocess_clip(desc, n, self.size, self.mean.ctypes.data, self.std.ctypes.data,
                                            self._ws.data_ptr(), self._ws.numel(), out.data_ptr(),
                                            int(self.dtype == torch.float16), current_stream_ptr()), "pg_preprocess_clip")
         return out
 
-    def __call__(self, images=None, return_tensors: str = "pt", square_crop: bool = False, **kwargs):
+    def __call__(self, images=None, return_tensors: str = "pt", square_crop: bool = False,
+                 windows: Optional[Sequence[CropWindow]] = None, fills: Optional[Sequence[Optional[tuple]]] = None,
+                 **kwargs):
+        """`windows` (one CropWindow per image) cuts each image to its rectangle first, `fills` gives each the RGB of
+        samples outside the image (default black).  A fill of None stands for padding that is no single RGB colour
+        (a CMYK file, say): that image is cropped by Pillow on the host (`_host_window`)."""
         if images is None:
             raise ValueError("You have to specify images.")
         if not isinstance(images, (list, tuple)):
             images = [images]
+        if windows is not None:
+            return {"pixel_values": self._windowed(images, windows, fills, square_crop)}
+        return {"pixel_values": self.preprocess_device(self._decode(images, square_crop))}
+
+    def _windowed(self, images, windows, fills, square_crop: bool) -> torch.Tensor:
+        n = len(images)
+        if square_crop:
+            raise ValueError("square_crop and windows do not combine")
+        fills = [(0, 0, 0)] * n if fills is None else list(fills)
+        if len(windows) != n or len(fills) != n:
+            raise ValueError(f"{n} images, {len(windows)} windows and {len(fills)} fills")
+        first, uniq, which = {}, [], [None] * n          # one decode per distinct file object
+        for i, (img, fill) in enumerate(zip(images, fills)):
+            if fill is None:
+                continue
+            if id(img) not in first:
+                first[id(img)] = len(uniq)
+                uniq.append(img)
+            which[i] = first[id(img)]
+        dev = self._decode(uniq, False)
+        crops, wins = [], []
+        for i, (w, fill) in enumerate(zip(windows, fills)):
+            w = CropWindow(*w)
+            if fill is None:
+                from PIL import Image
+                img = images[i]
+                if isinstance(img, (bytes, bytearray, memoryview)):
+                    img = Image.open(io.BytesIO(bytes(img)))
+                    self.host_decoded += 1
+                a = _host_window(img, w)
+                crops.append(torch.from_numpy(a).pin_memory().to(self.device, non_blocking=True))
+                wins.append((0, 0, a.shape[1], a.shape[0], (0, 0, 0)))
+                continue
+            t = _clip(dev[which[i]], w)
+            if t.shape[0] == 0 or t.shape[1] == 0:
+                raise ValueError(f"image {i}: the clip {w.clip} leaves no pixels")
+            crops.append(t)
+            wins.append((w.x0, w.y0, w.width, w.height, fill))
+        return self.preprocess_device(crops, wins)
+
+    def _decode(self, images, square_crop: bool) -> List[torch.Tensor]:
+        """Every image as a CUDA uint8 [H, W, 3] tensor (JPEGs, and PNGs with `png`, decoded on the GPU)."""
         dev = [None] * len(images)
         gpu_idx, gpu_files, gpu_infos = [], [], []
         png_idx, png_files, png_infos = [], [], []
@@ -183,4 +280,4 @@ class ClipImageProcessor:
                     if square_crop:
                         t = _square(t)
                 dev[i] = t
-        return {"pixel_values": self.preprocess_device(dev)}
+        return dev

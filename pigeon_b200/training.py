@@ -169,14 +169,16 @@ def schedule_lengths(num_examples: int, batch_size: int, grad_acc: int, world: i
     return len_dataloader, updates_per_epoch, total, warmup, n_epochs
 
 
-def pretrain(model: Any, dataset, train_args=None, resume: bool = False, data_collator: Optional[Callable] = None):
+def pretrain(model: Any, dataset, train_args=None, resume: bool = False, data_collator: Optional[Callable] = None,
+             trainer_cls=None):
     """reference training/train_modes.py:30-64: contrastive pretraining of a CLIPModel with the HF Trainer's loop
     (`pretrain.CLIPPretrainer`).  `model`: a `pigeon_b200.CLIPModel`, an HF `CLIPModel`, or a local directory / HF name.
     `dataset['train']` / `dataset['val']` hold rows with pixel_values, input_ids (and attention_mask).  The validation
     accuracy at batch size 16 is printed before and after training when the split has `.accuracy`.
 
     Unlike the reference, which calls `trainer.train` only under `if resume:`, this always trains; `resume` resumes from
-    `train_args.resume_from_checkpoint` (None = start fresh, True = the latest checkpoint in output_dir)."""
+    `train_args.resume_from_checkpoint` (None = start fresh, True = the latest checkpoint in output_dir).
+    `trainer_cls` replaces `CLIPPretrainer` (pretrain_data.FilesPretrainer trains from image files)."""
     from .clip_model import CLIPModel
     from .pretrain import CLIPPretrainer
     if train_args is None:
@@ -186,8 +188,9 @@ def pretrain(model: Any, dataset, train_args=None, resume: bool = False, data_co
     elif not isinstance(model, CLIPModel):
         model = CLIPModel.from_hf(model)
     model = model.to('cuda')
-    trainer = CLIPPretrainer(model, train_args, dataset['train'], eval_dataset=dataset['val'] if 'val' in dataset else None,
-                             data_collator=data_collator)
+    trainer = (trainer_cls or CLIPPretrainer)(model, train_args, dataset['train'],
+                                              eval_dataset=dataset['val'] if 'val' in dataset else None,
+                                              data_collator=data_collator)
     val = dataset['val'] if 'val' in dataset else None
     if hasattr(val, 'accuracy'):
         print('Before traing: Accuracy on batch size of 16 is', val.accuracy(model, batch_size=16))

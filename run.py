@@ -9,11 +9,15 @@
     python run.py finetune - -l EMBEDDING_DATASET_DIR --embeddings [-m]                          # head on embeddings (:171-175)
 
     python run.py pretrain openai/clip-vit-large-patch14-336 -l PRETRAIN_DATASET_DIR [--yfcc] [-r]          # (run.py:154-163)
+    python run.py pretrain openai/clip-vit-large-patch14-336 -l META.csv [--yfcc] [-a] [-r] [-w WORKERS] [--tokenizer DIR]
 
 `pretrain` trains a CLIPModel contrastively with the HF Trainer loop of `pretrain.CLIPPretrainer` (PRETAIN_ARGS, or
 PRETAIN_ARGS_YFCC with --yfcc; -r passes its `resume_from_checkpoint` to the trainer, as the reference does).  Its dataset is a pre-processed
-`DatasetDict` with `train` and `val` splits whose rows hold pixel_values, input_ids and attention_mask; the caption synthesis
-of the reference's PretrainDataset is not part of this repository.  Datasets are HF `DatasetDict`s on disk, as in the
+`DatasetDict` with `train` and `val` splits whose rows hold pixel_values, input_ids and attention_mask, or, when -l names a
+`.csv` file, the reference's pretraining metadata (run.py:106-110): `pretrain_data.PretrainDataset` (PretrainDatasetYFCC
+with --yfcc) synthesises the captions (-a adds the auxiliary sentences), CLIPTokenizer from --tokenizer (a local directory,
+config.CLIP_TOKENIZER_PATH by default) tokenises them, and the image files are decoded, cropped and pre-processed on the GPU
+batch by batch; -w worker processes read the files.  Datasets are HF `DatasetDict`s on disk, as in the
 reference (run.py:143-162); none are shipped with either repository.
 
 `finetune` trains the tower and head (`training.finetune_model`).  A split whose rows hold encoded `image` columns
@@ -109,15 +113,19 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument('--landmarks', action='store_true')
     p.add_argument('--heading', action='store_true')
     p.add_argument('-m', '--multitask', action='store_true')
+    p.add_argument('-a', '--auxiliary', action='store_true',
+                   help='pretrain from a metadata CSV: add the auxiliary caption sentences (climate, driving side, ...)')
+    p.add_argument('--tokenizer', default=cfg.CLIP_TOKENIZER_PATH,
+                   help='pretrain from a metadata CSV: local directory of the CLIP tokenizer files')
     p.add_argument('--embeddings', action='store_true', help='finetune: train the head on pre-computed embeddings')
     p.add_argument('--jpeg-multiscan', action='store_true',
-                   help='embed / finetune: decode progressive and multi-scan JPEGs on the GPU too (by default Pillow '
+                   help='embed / finetune / pretrain: decode progressive and multi-scan JPEGs on the GPU too (by default Pillow '
                         'decodes them)')
     p.add_argument('--png', action='store_true',
-                   help='embed / evaluate / finetune: decode PNG files on the GPU too (by default Pillow decodes them)')
+                   help='embed / evaluate / finetune / pretrain: decode PNG files on the GPU too (by default Pillow decodes them)')
     p.add_argument('-w', '--workers', type=int, default=0,
-                   help='evaluate / finetune: DataLoader worker processes (they read the image files of a benchmark or '
-                        'raw split)')
+                   help='evaluate / finetune / pretrain: DataLoader worker processes (they read the image files of a '
+                        'benchmark, raw split or pretraining CSV)')
     p.add_argument('--metrics', action='store_true',
                    help='evaluate / finetune: report compute_geoguessr_metrics (needs config.COUNTRY_PATH)')
     return p
@@ -143,6 +151,12 @@ def main(argv=None):
     if args.load is None:
         raise NotImplementedError('A dataset must be given with -l (the reference regenerates it from un-shipped raw data).')
     load = args.load.split(',')[0]
+    if args.mode == 'pretrain' and load.endswith('.csv'):
+        from pigeon_b200.pretrain_data import pretrain_files
+        pretrain_files(args.name, load, yfcc=args.yfcc, auxiliary=args.auxiliary, resume=args.resume,
+                       num_workers=args.workers, tokenizer=args.tokenizer, png=args.png,
+                       jpeg_multiscan=args.jpeg_multiscan)
+        return
     if args.mode == 'evaluate' and not os.path.isdir(load) and os.path.isfile(cfg.BENCHMARKS):   # run.py:158-162
         from pigeon_b200.benchmark import BenchmarkDataset
         print(evaluate(args.name, BenchmarkDataset(load), args.yfcc, args.landmarks, base_model=args.base,
