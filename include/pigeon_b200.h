@@ -155,7 +155,8 @@ size_t pg_head_workspace_bytes(int32_t B, int32_t D);
 /* emb f32 [B, V, D] (V = 4 for panoramas, 1 otherwise)
  *   -> pooled f32 [B, D]; logits f32 [B, C]; probs f32 [B, C]; pred_cell i64 [B];
  *      pred_lnglat f64 [B, 2] = centroids[pred_cell] (lng, lat);
- *      topk_val f32 [B, k] (descending), topk_idx i64 [B, k]. */
+ *      topk_val f32 [B, k] (descending), topk_idx i64 [B, k].
+ * B = 0 returns 0 at once and launches nothing; the pointers may then be NULL. */
 int pg_head_forward(const float* emb, int32_t B, int32_t V, int32_t D, const void* w3, const float* bias,
                     const double* centroids, int32_t C, int32_t k, void* workspace, size_t workspace_bytes,
                     float* pooled, float* logits, float* probs, int64_t* pred_cell, double* pred_lnglat,

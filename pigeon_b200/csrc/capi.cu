@@ -259,9 +259,12 @@ int pg_head_forward(const float* emb, int32_t B, int32_t V, int32_t D, const voi
                     const double* centroids, int32_t C, int32_t k, void* workspace, size_t workspace_bytes,
                     float* pooled, float* logits, float* probs, int64_t* pred_cell, double* pred_lnglat,
                     float* topk_val, int64_t* topk_idx, void* stream_) {
+  if (B < 0) { set_last_error("pg_head_forward: negative batch B=%d", B); return 1; }
+  // An empty batch has nothing to read or write, and zero-byte buffers may well be NULL (torch.empty(0).data_ptr() is 0),
+  // so it returns before the pointer checks (tests/test_gpu_head.py::test_head_empty_batch).
+  if (B == 0) return 0;
   if (!emb || !w3 || !centroids || !workspace || !pooled || !logits || !probs || !pred_cell || !pred_lnglat ||
       !topk_val || !topk_idx) { set_last_error("pg_head_forward: null argument"); return 1; }
-  if (B <= 0) return 0;
   if (V <= 0 || D % 8 || C <= 0 || k <= 0 || k > C) { set_last_error("pg_head_forward: bad shape B=%d V=%d D=%d C=%d k=%d", B, V, D, C, k); return 1; }
   if (workspace_bytes < pg_head_workspace_bytes(B, D)) { set_last_error("pg_head_forward: workspace too small"); return 1; }
   const int sms = sm_count();
