@@ -1,5 +1,5 @@
 """Constants of the hot path, same names and values as the reference's config.py (file:line cited per block).
-Only what the hot path and the fine-tune step read is mirrored; dataset-creation paths are out of scope."""
+Only what the hot path, the dataset builders and the training steps read is mirrored."""
 from types import SimpleNamespace
 
 # OpenAI's pretrained implementation                                   (config.py:5-7)
@@ -15,6 +15,12 @@ IMAGE_PATH_YFCC = 'data/images_mp_16/jpgs'
 DRIVING_SIDE_PATH = 'data/driving_side/countries_driving_side.json'
 # A local copy of CLIP_MODEL's tokenizer files (vocab.json, merges.txt): nothing is downloaded
 CLIP_TOKENIZER_PATH = 'saved_models/clip_tokenizer'
+
+# Fine-tuning data: metadata CSVs and image folders                     (config.py:10, 12, 17, 19, 22-23)
+METADATA_PATH = 'data/data_duels.csv'
+METADATA_PATH_YFCC = 'data/data_yfcc_augmented_non_contaminated.csv'
+METADATA_PATH_LANDMARKS = 'data/data_landmarks_aug.csv'
+IMAGE_PATH_LANDMARKS = 'data/benchmarks/google_landmark/jpgs'
 
 # Geocells path                                                        (config.py:34-36)
 GEOCELL_PATH = 'data/geocells_2203.csv'       # PIGEON
